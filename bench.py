@@ -3,7 +3,7 @@
 
 Workload (BASELINE.json configs[2], the one the metric is quoted on; it fits one GPU): 100k queries x 1M-row
 index, 768-d bf16, K=32, synthetic L2-normalised Gaussian embeddings (corpus seed 0, queries seed 1). A "step" is
-one pass of the hot path over the whole query batch: `VS.__call__` of the sim-join (fused tcgen05 filter + exact
+one pass of the hot path over the whole query batch: `VS.__call__` of the sim-join (fused wgmma filter + exact
 finalize [+ all-gather + k-way merge when the index is row-sharded over N GPUs]).
 
     python bench.py --gpus 1 --steps 5 --warmup 3
@@ -15,9 +15,14 @@ finalize [+ all-gather + k-way merge when the index is row-sharded over N GPUs])
 Prints ONE JSON line (rank 0). `value` = device-resident throughput; `e2e` = the plugin's own host-buffer call
 (b2_index_search at N=1: pinned host queries in, host scores + ids out, H2D/D2H inside; at N>1 ShardedIndex.search_host: each
 rank copies 1/N of the queries over PCIe, the ranks all-gather them over NVLink); `operator_e2e` = DataFrame in -> DataFrame
-out through the pandas accessor (N=1); `roofline` is the tcgen05 filter kernel against the measured dense bf16 peak
-(MEASURED_PEAKS.json); `cpu_baseline` is the CPU arm on a bounded sample of the same workload; `parity` compares the (merged)
+out through the pandas accessor (N=1); `roofline` is the wgmma filter kernel against the H100 SXM data-sheet dense bf16
+rate (989 TFLOP/s at 700 W; `clocks` records the card's name and power limit); `cpu_baseline` is the CPU arm on a bounded sample of the same workload; `parity` compares the (merged)
 GPU result with the canonical oracle on 256 queries at EVERY N and says which oracle ran ("faiss" when the wheel is importable).
+
+    --dump-outputs DIR   after the timed steps, writes what the last timed step returned: DIR/scores.npy (float32 [nq, k]) and
+                         DIR/indices.npy (float64 [nq, k]); inputs are seeded, so two builds can be compared output for output.
+                         Above 64 MB in all, a fixed seeded sample of query rows is written instead, with DIR/rows.npy (float64)
+                         holding which rows. Headline configuration (c3) of the GPU arm only.
 """
 from __future__ import annotations
 
@@ -35,6 +40,7 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
 BLOCK_ROWS = 1 << 16  # data is generated in fixed row blocks so every world size sees the same matrix
+DUMP_LIMIT_BYTES = 64 << 20  # --dump-outputs writes at most this much
 
 
 def env_int(name: str, default: int) -> int:
@@ -78,17 +84,23 @@ def to_bf16_values(a: np.ndarray) -> np.ndarray:
 
 
 class ClockSampler:
-    """nvidia-smi sampling DURING the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi sampling DURING the timed region: SM clock, power draw, throttle reasons; plus the card's name and power limit."""
 
     def __init__(self, gpu_index: int):
         self.gpu = gpu_index
         self.lines: list[str] = []
         self.proc = None
         self.thread = None
+        self.card = None
 
     def start(self):
         q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
              "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
+        try:
+            self.card = subprocess.run(["nvidia-smi", f"--id={self.gpu}", "--query-gpu=name,power.limit", "--format=csv,noheader"],
+                                       capture_output=True, text=True, timeout=30).stdout.strip()
+        except Exception:
+            self.card = None
         try:
             self.proc = subprocess.Popen(["nvidia-smi", f"--id={self.gpu}", f"--query-gpu={q}", "--format=csv,noheader,nounits",
                                           "-lms", "50"], stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True)
@@ -106,7 +118,7 @@ class ClockSampler:
 
     def stop(self) -> dict:
         if self.proc is None:
-            return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
+            return {"sm_mhz": None, "sm_max_mhz": None, "card": self.card, "reasons": ["nvidia-smi unavailable"]}
         self.proc.terminate()
         try:
             self.proc.wait(timeout=5)
@@ -128,19 +140,11 @@ class ClockSampler:
                 if val.lower().startswith("active"):
                     reasons.add(nm)
         return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": max(mx) if mx else None,
-                "power_w_max": max(power) if power else None, "samples": len(sm), "reasons": sorted(reasons)}
+                "power_w_max": max(power) if power else None, "card": self.card, "samples": len(sm), "reasons": sorted(reasons)}
 
 
 def load_peaks() -> tuple[float, str]:
-    path = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    try:
-        with open(path) as f:
-            pk = json.load(f)
-        if "bf16_tflops_sustained" in pk:
-            return float(pk["bf16_tflops_sustained"]), "measured bf16_tflops_sustained (MEASURED_PEAKS.json; kernel timed inside a long step)"
-        return float(pk["bf16_tflops"]), "measured bf16_tflops (MEASURED_PEAKS.json)"
-    except Exception:
-        return 1590.0, "fallback 1.59 PFLOP/s (B200_PROFILING.md; MEASURED_PEAKS.json absent)"
+    return 989.0, "H100 SXM data sheet, dense bf16 at 700 W (not measured; a lower power limit lowers it)"
 
 
 # ---- CPU arms ------------------------------------------------------------------------------------------------------------------
@@ -308,7 +312,7 @@ def reference_operator_leg(args, x: np.ndarray, q: np.ndarray, k: int) -> dict:
         t_join = time.perf_counter() - t0
     return {"value": len(q) / t_join, "unit": "queries/s", "seconds": t_join, "rows_out": int(len(out)), "left_rows": len(q), "right_rows": len(x),
             "sem_index_seconds_both_frames": t_index, "faiss": faiss_kind,
-            "what": "reference lotus/sem_ops/sem_sim_join.py + lotus/vector_store/faiss_vs.py, unmodified (baseline/_ref)"}
+            "what": "reference lotus/sem_ops/sem_sim_join.py + lotus/vector_store/faiss_vs.py, unmodified (oracle/_ref)"}
 
 
 def run_reference(args) -> None:
@@ -357,11 +361,11 @@ def run_reference(args) -> None:
         "impl": "reference", "metric": "sem_sim_join queries/sec (1M x 768, K=32)", "value": val, "unit": "queries/s",
         "n_gpus": args.gpus, "steps": args.steps, "warmup": args.warmup, "ms_per_step": dt * 1e3,
         "higher_is_better": True, "scaling": "strong", "vs_baseline": None, "dtype": "f32 (bf16 values)", "data": "synthetic",
-        # same keys and workload string as the B200 arm's `config`; what is specific to this run sits in `reference_run`
+        # same keys and workload string as the GPU arm's `config`; what is specific to this run sits in `reference_run`
         "config": {"workload": f"sem_sim_join {args.nq} queries x {n} index, {d}-d bf16, K={k} (BASELINE.json configs[2])", "nq": args.nq,
                    "n": n, "d": d, "k": k, "parallelism": f"{arms['cores']} host threads (no GPU)", "l2_policy": "n/a (CPU arm)"},
         "reference_run": {"sample_queries_per_step": sample, "datagen_s": round(gen_s, 1), "tflops": 2.0 * n * d * val / 1e12,
-                          "data": "same generator, distribution and seeds as the B200 arm (numpy stream instead of the CUDA one)"},
+                          "data": "same generator, distribution and seeds as the GPU arm (numpy stream instead of the CUDA one)"},
         "cpu_baseline": arms, "oracle": probe,
         "e2e": {"value": val, "unit": "queries/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
         "operator_e2e": op,
@@ -371,7 +375,7 @@ def run_reference(args) -> None:
 
 
 def operator_leg(torch, nv, corpus, queries, k: int, reps: int = 2) -> dict:
-    """Operator scope on the B200 (SURVEY §8d-ii): DataFrame in -> DataFrame out through the pandas accessor
+    """Operator scope on the GPU (SURVEY §8d-ii): DataFrame in -> DataFrame out through the pandas accessor
     (lotus_b200/sem_ops/sem_sim_join.py: same control flow as the reference's, B200VS underneath), next to the VS boundary."""
     import tempfile
 
@@ -436,7 +440,11 @@ def main() -> None:
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-operator", action="store_true", help="skip the DataFrame -> DataFrame leg")
     ap.add_argument("--parity-queries", type=int, default=256)
+    ap.add_argument("--dump-outputs", type=str, default=None, metavar="DIR",
+                    help="write the last timed step's scores and indices as DIR/scores.npy (float32) and DIR/indices.npy (float64)")
     args, extra = ap.parse_known_args()
+    if args.dump_outputs and (args.config != "c3" or args.impl == "reference"):
+        ap.error("--dump-outputs writes the GPU arm's headline-configuration outputs: use it without --config / --impl reference")
     if args.warmup < 3:
         args.warmup = 3
     if args.config != "c3":
@@ -494,9 +502,10 @@ def main() -> None:
         return float(ms.item()) / steps
 
     filt_ms: list[float] = []
+    last_out: list = [None]
 
     def step_dev():
-        index.search(queries, k)
+        last_out[0] = index.search(queries, k)
         filt_ms.append(index.last_filter_ms())
 
     # ---- device-resident throughput --------------------------------------------------------------------------------
@@ -509,6 +518,18 @@ def main() -> None:
         sampler.start()
     ms_step = timed(step_dev, args.steps)
     clocks = sampler.stop() if sampler else None
+    if args.dump_outputs and rank == 0 and last_out[0] is not None:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        s_last, i_last = last_out[0]
+        if nq * k * 12 > DUMP_LIMIT_BYTES:  # float32 scores + float64 indices per entry; rows.npy adds 8 bytes per kept row
+            keep = DUMP_LIMIT_BYTES // (k * 12 + 8)
+            rows = np.sort(np.random.default_rng(0).choice(nq, keep, replace=False))
+            rows_dev = torch.from_numpy(rows).to(s_last.device)
+            s_last, i_last = s_last[rows_dev], i_last[rows_dev]
+            np.save(os.path.join(args.dump_outputs, "rows.npy"), rows.astype(np.float64))
+        np.save(os.path.join(args.dump_outputs, "scores.npy"), s_last.float().cpu().numpy())
+        np.save(os.path.join(args.dump_outputs, "indices.npy"), i_last.cpu().numpy().astype(np.float64))
+    last_out[0] = None
     st = nv.stats()
     launches_per_step = st["launches"] / max(args.steps, 1) + (1 if world > 1 else 0)  # + the all-gather kernel is NCCL's
     fallback_q = st["fallback_queries"]
@@ -564,24 +585,16 @@ def main() -> None:
                    "sharded search, rank 0 copies the merged result D2H; CUDA events, max over ranks")
         h2d_rank = h2d // world
 
-    # ---- roofline of the dominant kernel (the tcgen05 filter), per rank-0 launch --------------------------------------
+    # ---- roofline of the dominant kernel (the wgmma filter), per rank-0 launch ----------------------------------------
     peak_tf, peak_src = load_peaks()
     flops_launch = 2.0 * nq * (hi - lo) * d  # algorithmic: 2*N_local*d per query (SURVEY §8d)
     achieved_tf = flops_launch / (kernel_ms * 1e-3) / 1e12 if kernel_ms == kernel_ms and kernel_ms > 0 else None
-    traffic = None
-    try:  # DRAM bytes of one launch of this kernel on this shape, from the committed `ncu --set full` capture
-        with open(os.path.join(ROOT, "profiles", "filter_traffic.json")) as f:
-            tj = json.load(f)
-        if tj.get("nq") == nq and tj.get("n_local") == hi - lo and tj.get("d") == d:
-            traffic = tj["dram_bytes_read"] + tj["dram_bytes_write"]
-    except Exception:
-        traffic = None
     roofline = {"bound": "tensor", "achieved": achieved_tf, "peak": peak_tf, "unit": "TFLOP/s",
-                "frac": (achieved_tf / peak_tf) if achieved_tf else None, "traffic": traffic,
-                "kernel": "knn_filter_kernel<KP=64,IP,bf16,cta_group::2>", "kernel_ms": kernel_ms, "peak_source": peak_src,
+                "frac": (achieved_tf / peak_tf) if achieved_tf else None,
+                "kernel": "knn_filter_kernel<KP=64,IP,bf16,CTA pair>", "kernel_ms": kernel_ms, "peak_source": peak_src,
                 "kernel_ms_per_rank": [round(v, 3) for v in kernel_ms_ranks],
                 "algorithmic_flops_per_launch": flops_launch,
-                "hbm_floor_ms": ((hi - lo) * d * 2 + nq * d * 2 + nq * k * 12) / 6.4843e12 * 1e3}
+                "hbm_floor_ms": ((hi - lo) * d * 2 + nq * d * 2 + nq * k * 12) / 3.35e12 * 1e3}  # H100 SXM data-sheet HBM3 rate
 
     # ---- parity at every N: the (merged) result of 256 queries against the canonical oracle, indices and score bits ----------
     parity = None
@@ -649,7 +662,7 @@ def main() -> None:
             "higher_is_better": True, "scaling": "strong", "vs_baseline": None, "dtype": "bf16", "data": "synthetic",
             "config": {"workload": f"sem_sim_join {nq} queries x {n} index, {d}-d bf16, K={k} (BASELINE.json configs[2])",
                        "nq": nq, "n": n, "d": d, "k": k, "parallelism": f"index row-sharded x{world}",
-                       "l2_policy": "inputs exceed L2 (corpus shard %.0f MB + queries %.0f MB vs 126 MB L2)" %
+                       "l2_policy": "inputs exceed L2 (corpus shard %.0f MB + queries %.0f MB vs 50 MB L2)" %
                                     ((hi - lo) * d * 2 / 1e6, nq * d * 2 / 1e6)},
             "e2e": {"value": nq / (ms_e2e * 1e-3), "unit": "queries/s", "ms_per_step": ms_e2e,
                     "h2d_bytes_per_step": h2d_rank, "d2h_bytes_per_step": d2h, "api": e2e_api},

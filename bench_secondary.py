@@ -2,7 +2,7 @@
 (`python bench.py --config cX --gpus N --steps K --warmup W`, torchrun for N > 1, one JSON line from rank 0 with metric / value /
 unit / roofline / cpu_baseline / parity / e2e / clocks):
 
-  c2  sem_search over a 1M x 768 fp32 index, 10k queries, top-10 (TF32 tcgen05 filter + exact fp32 re-score); index row-sharded at N > 1
+  c2  sem_search over a 1M x 768 fp32 index, 10k queries, top-10 (TF32 wgmma filter + exact fp32 re-score); index row-sharded at N > 1
   c4  sem_dedup relation, 10M rows x 384-d bf16, cosine > 0.95, 1 % planted near-duplicates; corpus replicated, the upper-triangular
       tile grid dealt over max(N, --dedup-parts) parts (at N = 1 the default times ONE rank's share of the 8-GPU split)
   c5  sem_cluster_by k-means, 5M x 768 bf16, k = 1024, 20 Lloyd iterations + final assignment; points row-sharded at N > 1
@@ -21,10 +21,8 @@ import bench
 
 
 def _peaks():
-    try:
-        return json.load(open(os.path.join(bench.ROOT, "MEASURED_PEAKS.json")))
-    except Exception:
-        return {"bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "hbm_gbs": 6650.0}
+    # H100 SXM data sheet at 700 W (not measured): dense bf16 TFLOP/s and HBM3 GB/s
+    return {"bf16_tflops": 989.0, "hbm_gbs": 3350.0}
 
 
 class Ctx:
@@ -146,7 +144,7 @@ def c2(ctx: Ctx, extra):
             for key in ("_sample", "_I", "_D"):
                 cpu.pop(key, None)
         pk = _peaks()
-        peak = pk.get("bf16_tflops_sustained", pk["bf16_tflops"]) / 2.0
+        peak = pk["bf16_tflops"] / 2.0
         fl = 2.0 * nq * (hi - lo) * d
         line = _base(ctx, "sem_search queries/sec (1M x 768 fp32, top-10)", nq / ms * 1e3, "queries/s", ms, True, "f32 (tf32 filter, exact fp32 re-score)",
                      {"workload": f"sem_search {nq} queries x {n} index, {d}-d fp32, K={k} (BASELINE.json configs[1])", "nq": nq, "n": n, "d": d, "k": k,
@@ -156,8 +154,8 @@ def c2(ctx: Ctx, extra):
                              "d2h_bytes_per_step": nq * k * 12, "api": api},
                      "gpu_launches": int(st["launches"]), "fallback_queries": int(st["fallback_queries"]),
                      "roofline": {"bound": "tensor", "achieved": fl / kms / 1e9, "peak": peak, "unit": "TFLOP/s", "frac": fl / kms / 1e9 / peak, "traffic": None,
-                                  "kernel": "knn_filter_kernel<KP=32,IP,tf32,cta_group::2>", "kernel_ms": kms,
-                                  "peak_source": "half the measured sustained bf16 figure (kind::tf32 issues at half the kind::f16 rate; no TF32 entry in MEASURED_PEAKS.json)"},
+                                  "kernel": "knn_filter_kernel<KP=32,IP,tf32,CTA pair>", "kernel_ms": kms,
+                                  "peak_source": "H100 SXM data-sheet dense tf32 rate (half the bf16 rate; not measured)"},
                      "cpu_baseline": cpu, "parity": parity, "clocks": clocks})
     index.close()
     ctx.finish(line)
@@ -249,7 +247,7 @@ def c4(ctx: Ctx, extra):
                    "sample": f"{ns} x {ns} x {d} all-pairs scores in {dt:.2f} s (orc_knn_tiled, -march=native), scaled by (n/ns)^2/2"
                              f"{' x this share' if share < 1 else ''}: an ESTIMATE — the reference materialises an N^2-row DataFrame (sem_dedup.py:45) and cannot run at this size"}
         pk = _peaks()
-        peak = pk.get("bf16_tflops_sustained", pk["bf16_tflops"])
+        peak = pk["bf16_tflops"]
         fl = float(n) * (n - 1) / 2 * 2 * d / (nparts if ctx.world == 1 else ctx.world)
         share_txt = f"one rank's share (part 0 of {nparts})" if ctx.world == 1 and nparts > 1 else f"tile grid dealt over {ctx.world} ranks"
         line = _base(ctx, "sem_dedup seconds (10M x 384, cosine > 0.95)", ms / 1e3, "s", ms, False, "bf16",
@@ -261,7 +259,7 @@ def c4(ctx: Ctx, extra):
                                     + ("; + all-gather of the per-rank lists)" if ctx.world > 1 else ")")},
                      "gpu_launches": int(st["launches"]),
                      "roofline": {"bound": "tensor", "achieved": fl / ms / 1e9, "peak": peak, "unit": "TFLOP/s", "frac": fl / ms / 1e9 / peak, "traffic": None,
-                                  "kernel": "pair_filter_kernel<bf16,cta_group::2>", "kernel_ms": ms,
+                                  "kernel": "pair_filter_kernel<bf16,CTA pair>", "kernel_ms": ms,
                                   "note": "whole call timed (filter + verify + sort + D2H): the filter kernel is > 95 % of it; symmetric FLOP count N(N-1)/2*2d"},
                      "cpu_baseline": cpu, "parity": parity, "clocks": clocks})
     idx.close()
@@ -351,7 +349,7 @@ def c5(ctx: Ctx, extra):
                    "sample": f"oracle.kmeans (canonical fp64 scorer, OpenMP) on {ns} points x {ks} centroids: {per_it:.3f} s/iteration, scaled by n*k to "
                              f"{n} x {k}: an ESTIMATE (faiss's sgemm path would be faster than this scalar port)"}
         pk = _peaks()
-        peak = pk.get("bf16_tflops_sustained", pk["bf16_tflops"])
+        peak = pk["bf16_tflops"]
         npts = (n if full else min(n, 256 * k))
         passes_fl = 2.0 * k * d * (npts * niter + n) / ctx.world
         s_per_it = ms / 1e3 / (niter + 1)
@@ -365,9 +363,9 @@ def c5(ctx: Ctx, extra):
                              if ctx.world == 1 else "sharded_kmeans (b2_kmeans_assign_dev + b2_kmeans_accumulate_dev + NCCL all-reduce per iteration)"},
                      "gpu_launches": int(st["launches"]), "second_level_points": int(st["fallback_queries"]),
                      "roofline": {"bound": "tensor", "achieved": passes_fl / ms / 1e9, "peak": peak, "unit": "TFLOP/s", "frac": passes_fl / ms / 1e9 / peak,
-                                  "traffic": None, "kernel": "knn_filter_kernel<16,L2,bf16,cta_group::2,TOP1> (+ update pass)", "kernel_ms": ms,
+                                  "traffic": None, "kernel": "knn_filter_kernel<16,L2,bf16,CTA pair,TOP1> (+ update pass)", "kernel_ms": ms,
                                   "note": "whole run timed: 2*n*k*d FLOP per assignment pass; the centroid update adds one HBM pass over the points per iteration "
-                                          "(n*d*2 bytes = %.2f ms at the measured %.0f GB/s)" % ((hi - lo) * d * 2 / pk.get("hbm_gbs", 6650.0) / 1e6, pk.get("hbm_gbs", 6650.0))},
+                                          "(n*d*2 bytes = %.2f ms at the data-sheet %.0f GB/s)" % ((hi - lo) * d * 2 / pk["hbm_gbs"] / 1e6, pk["hbm_gbs"])},
                      "cpu_baseline": cpu, "parity": parity, "clocks": clocks})
     idx.close()
     ctx.finish(line)

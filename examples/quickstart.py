@@ -1,4 +1,4 @@
-"""The five embedding operators of LOTUS on a B200 through lotus_b200 (needs a B200; there is no CPU path).
+"""The five embedding operators of LOTUS on an H100 through lotus_b200 (needs an H100; there is no CPU path).
 
 With the real `lotus` package installed the only change to an existing script is the vector store:
 

@@ -1,5 +1,5 @@
 /*
- * lotus_b200.h — C-ABI of libb2lotus.so, the B200 (sm_100a) vector-store backend for LOTUS.
+ * lotus_b200.h — C-ABI of libb2lotus.so, the H100 (sm_90a) vector-store backend for LOTUS.
  *
  * This is the drop-in boundary for ONE hot path of lotus-data/lotus: the faiss-backed
  * `lotus.vector_store.FaissVS` and the faiss.Kmeans call in `lotus.utils.cluster`.
@@ -75,7 +75,7 @@ typedef struct b2_index b2_index;
 /* ---- library ---------------------------------------------------------------------------------------- */
 B2_API int b2_abi_version(void);
 B2_API const char* b2_last_error(void);
-/* number of visible CUDA devices that are sm_100 (B200); 0 when there is none */
+/* number of visible CUDA devices that are sm_90 (H100); 0 when there is none */
 B2_API int b2_device_count(void);
 /* largest k supported by b2_index_search */
 B2_API int b2_max_k(void);
@@ -124,7 +124,7 @@ B2_API int b2_merge_topk_packed_dev(const uint64_t* packed_dev, const int64_t* s
                              int32_t metric, int32_t device, float* out_scores_dev, int64_t* out_idx_dev, void* stream);
 
 /* Row-sharded search in two stages, so that the ranks can tell each other how good the merged top k will be BEFORE the exact
- * re-scoring. Stage 1 filters this shard (tcgen05 kernel) and writes lower_dev[nq]: for every query a lower bound on the exact
+ * re-scoring. Stage 1 filters this shard (wgmma kernel) and writes lower_dev[nq]: for every query a lower bound on the exact
  * score of its j best local candidates (-inf when unknown); it only enqueues work on `stream`. The caller all-reduces (MIN)
  * lower_dev over the ranks with j = ceil(k / ranks) — k rows of the whole index are then known to reach that score — and hands
  * the result to stage 2, which re-scores only the local candidates that can still reach it (about k / ranks instead of k + 2),
@@ -198,12 +198,12 @@ B2_API int b2_debug_filter_plan(int64_t nq, int64_t n, int32_t k, int32_t num_sm
 
 /* ---- instrumentation ---------------------------------------------------------------------------------- */
 /* counters since the last b2_stats_reset(): [0] kernels launched by this library, [1] queries answered,
- * [2] queries that took the exact dense fallback, [3] tcgen05 filter launches, [4] rows rescored exactly,
+ * [2] queries that took the exact dense fallback, [3] wgmma filter launches, [4] rows rescored exactly,
  * [5] queries of fp32 indexes that the bf16 first-level filter could not certify and the tf32 level answered.
  * Returns how many counters were written (<= cap). */
 B2_API int b2_stats(int64_t* out, int32_t cap);
 B2_API void b2_stats_reset(void);
-/* device time (ms) of the dominant kernel (the tcgen05 filter) in the last search on this handle, measured
+/* device time (ms) of the dominant kernel (the wgmma filter) in the last search on this handle, measured
  * with CUDA events on the stream it was launched on; <0 when unavailable. */
 B2_API float b2_last_filter_ms(const b2_index* idx);
 

@@ -1,4 +1,4 @@
-"""lotus_b200 — B200-native (sm_100a) backend for the embedding-similarity hot path of lotus-data/lotus:
+"""lotus_b200 — H100-native (sm_90a) backend for the embedding-similarity hot path of lotus-data/lotus:
 `lotus.vector_store.FaissVS` + `sem_index / sem_search / sem_sim_join / sem_dedup / sem_cluster_by`.
 
     import lotus_b200 as lotus                      # same names as the reference for this path

@@ -1,5 +1,5 @@
 """ctypes binding of libb2lotus.so (include/lotus_b200.h). No CPU fallback: if the library is not built or no
-B200 is visible, calls raise — they never degrade to a host implementation."""
+H100 is visible, calls raise — they never degrade to a host implementation."""
 from __future__ import annotations
 
 import ctypes
@@ -114,10 +114,10 @@ def device_count() -> int:
 
 def require_device() -> None:
     if device_count() == 0:
-        raise RuntimeError("lotus_b200 needs a B200 (sm_100) GPU; none is visible and there is no CPU fallback")
+        raise RuntimeError("lotus_b200 needs an H100 (sm_90) GPU; none is visible and there is no CPU fallback")
 
 
-def filter_plan(nq: int, n: int, k: int, num_sms: int = 148) -> dict:
+def filter_plan(nq: int, n: int, k: int, num_sms: int = 132) -> dict:
     """The filter kernel's schedule for a shape (host logic only, no device needed)."""
     kp, ns, uw, two = ctypes.c_int32(), ctypes.c_int32(), ctypes.c_int32(), ctypes.c_int32()
     check(lib().b2_debug_filter_plan(nq, n, k, num_sms, ctypes.byref(kp), ctypes.byref(ns), ctypes.byref(uw), ctypes.byref(two)))
@@ -307,8 +307,8 @@ def _index_kmeans_accumulate_dev(self, assign_ptr: int, k: int, sums_ptr: int, c
 
 def pair_owner(i, nparts: int):
     """Rank that owns the pairs (i, j > i) in `threshold_pairs(part=, nparts=)`: 128-row query tiles are dealt to the ranks in
-    groups of one tile per SM (148 on B200; B2_PAIR_GROUP overrides) — mirrors launch_pair_filter in knn_filter_sm100.cu."""
-    group = int(os.environ.get("B2_PAIR_GROUP", "0")) or 148
+    groups of one tile per SM (132 on H100; B2_PAIR_GROUP overrides) — mirrors launch_pair_filter in knn_filter_sm90.cu."""
+    group = int(os.environ.get("B2_PAIR_GROUP", "0")) or 132
     tile = np.asarray(i, dtype=np.int64) // 128
     if int(os.environ.get("B2_PAIR_2CTA", "1")):  # CTA pairs (default): the unit is two consecutive query tiles, one unit per pair of SMs
         return ((tile // 2) // max(1, group // 2)) % nparts

@@ -1,4 +1,4 @@
-"""Build libb2lotus.so (sm_100a only) in-tree with nvcc. No torch, no CPU fallback.
+"""Build libb2lotus.so (sm_90a only) in-tree with nvcc. No torch, no CPU fallback.
 
     python -m lotus_b200.build [--force]
 
@@ -18,7 +18,7 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "csrc", "_obj")
 LIB = os.path.join(HERE, "libb2lotus.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-std=c++17", "-O3", "-lineinfo",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-std=c++17", "-O3", "-lineinfo",
          "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--expt-relaxed-constexpr",
          "-diag-suppress", "177"]
 
@@ -55,7 +55,7 @@ def build(force: bool = False) -> str:
             os.remove(f)
     with cf.ThreadPoolExecutor(max_workers=min(8, os.cpu_count() or 1)) as ex:
         objs = list(ex.map(_compile, sources()))
-    cmd = [NVCC, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB, *objs]
+    cmd = [NVCC, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", LIB, *objs]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         sys.stderr.write(r.stdout + r.stderr)

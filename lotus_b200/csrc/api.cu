@@ -1,5 +1,5 @@
 // api.cu — the C-ABI of libb2lotus.so (include/lotus_b200.h): handles, workspaces and the search pipeline
-//   prep queries -> tcgen05 filter (knn_filter_sm100.cu) -> finalize/certify (knn_exact.cu) -> dense exact
+//   prep queries -> wgmma filter (knn_filter_sm90.cu) -> finalize/certify (knn_exact.cu) -> dense exact
 //   fallback for uncertified queries.
 // Reference call sites replaced: lotus/vector_store/faiss_vs.py:22-77 (see the header for the mapping).
 #include <algorithm>
@@ -76,10 +76,10 @@ float filter_rel_eps(int store_dtype, int filt_dtype, int q_dtype, int d) {
     // tests/test_gpu_fuzz.py: a too-small bound shows up as a wrong neighbour, a too-large one only as fallback work.
     const double acc = (double)(d + 64) * 1.1920929e-7;
     double ex = 0.0, eq = 0.0;  // relative representation error of the corpus / query operand seen by the MMA
-    if (filt_dtype == B2_F32) {  // kind::tf32 keeps 10 explicit mantissa bits of an fp32 operand
+    if (filt_dtype == B2_F32) {  // tf32 wgmma keeps 10 explicit mantissa bits of an fp32 operand
         ex = store_dtype == B2_F32 ? 9.765625e-4 : 0.0;  // bf16 values are exact in tf32
         eq = q_dtype == B2_F32 ? 9.765625e-4 : 0.0;
-    } else {  // kind::f16 on bf16 operands
+    } else {  // bf16 wgmma on bf16 operands
         ex = store_dtype == B2_F32 ? 3.90625e-3 : 0.0;  // fp32 values rounded to bf16 for the filter
         eq = q_dtype == B2_F32 ? 3.90625e-3 : 0.0;
     }
@@ -118,7 +118,7 @@ int search_core(b2_index* idx, const MatView& X_in, int metric, const void* q_de
     if (nq <= 0) return B2_OK;
     if (level == 0) g_stats[ST_QUERIES] += nq;
     // candidate capacity of the bf16 first level (the 2^-8 operand error lets more rows straddle the k-th score): 0 = not used
-    const int kp16 = (X_in.filt16 && level == 0 && X_in.n >= 4096) ? (k <= 4 ? 32 : k <= 12 ? 64 : k <= 24 ? 96 : 0) : 0;
+    const int kp16 = (X_in.filt16 && level == 0 && X_in.n >= 4096) ? (k <= 4 ? 32 : k <= 12 ? 64 : k <= 24 ? 72 : 0) : 0;
     MatView X = X_in;
     if (kp16) {
         X.filt = X_in.filt16;
@@ -128,7 +128,7 @@ int search_core(b2_index* idx, const MatView& X_in, int metric, const void* q_de
     const bool defer = kp16 != 0;
     int64_t n_deferred = 0;
     if (X.n <= 0) {
-        fill_pad_kernel<<<148, 256, 0, st>>>(out_sc, out_id, nq * k, metric == B2_METRIC_L2 ? FLT_MAX : -FLT_MAX);
+        fill_pad_kernel<<<132, 256, 0, st>>>(out_sc, out_id, nq * k, metric == B2_METRIC_L2 ? FLT_MAX : -FLT_MAX);
         B2_LAUNCH_CHECK();
         return B2_OK;
     }
@@ -152,7 +152,7 @@ int search_core(b2_index* idx, const MatView& X_in, int metric, const void* q_de
         g_stats[ST_FALLBACK] += nq;
         return B2_OK;
     }
-    int dev_sms = 148;
+    int dev_sms = 132;
     cudaDeviceGetAttribute(&dev_sms, cudaDevAttrMultiProcessorCount, idx->device);
     const int filt_dtype = X.filt_dtype;
     const int64_t q_pitch = round_up(X.d, filt_dtype == B2_F32 ? 4 : 8);
@@ -277,9 +277,10 @@ int b2_device_count(void) {
     }
     int ok = 0;
     for (int i = 0; i < n; ++i) {
-        int major = 0;
+        int major = 0, minor = 0;
         cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, i);
-        if (major == 10) ok++;
+        cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, i);
+        if (major == 9 && minor == 0) ok++;
     }
     return ok;
 }
@@ -300,9 +301,10 @@ int b2_index_create(const void* x, int64_t n, int32_t d, int32_t dtype, int32_t 
         return B2_ENODEV;
     }
     if (device < 0 || device >= ndev) { set_error("device %d out of range (%d visible)", device, ndev); return B2_EINVAL; }
-    int major = 0;
+    int major = 0, minor = 0;
     cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device);
-    if (major != 10) { set_error("device %d is sm_%d0; this library is built for sm_100a (B200) only", device, major); return B2_ENODEV; }
+    cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, device);
+    if (major != 9 || minor != 0) { set_error("device %d is sm_%d%d; this library is built for sm_90a (H100) only", device, major, minor); return B2_ENODEV; }
     DeviceGuard guard(device);
     b2_index* idx = new b2_index();
     idx->device = device;
@@ -481,7 +483,7 @@ int b2_index_search_stage1_dev(b2_index* idx, const void* q_dev, int64_t nq, int
     const bool use_filter = kp != 0 && X.n >= 512 && ceil_div(X.n, 256) >= min_splits && X.n >= 4 * (int64_t)k;
     const bool two_level = X.filt16 != nullptr && k <= 24 && X.n >= 4096;
     const int64_t chunk = std::max<int64_t>(4096, std::min<int64_t>(1 << 20, (4LL << 30) / ((int64_t)std::max(min_splits, 8) * kp * 8)));
-    int dev_sms = 148;
+    int dev_sms = 132;
     cudaDeviceGetAttribute(&dev_sms, cudaDevAttrMultiProcessorCount, idx->device);
     const bool two_cta = filter_use_pair(nq);
     int units_whole = 0;

@@ -1,4 +1,4 @@
-// common.cuh — shared declarations for libb2lotus.so (sm_100a only).
+// common.cuh — shared declarations for libb2lotus.so (sm_90a only).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -78,7 +78,7 @@ __host__ __device__ __forceinline__ float best_first_unkey(uint32_t k, int metri
 }
 
 // ---- a matrix the kernels can search ---------------------------------------------------------------------
-// `store` holds the exact values (dtype f32 or bf16, row pitch `d`). `filt` is what the tcgen05 filter
+// `store` holds the exact values (dtype f32 or bf16, row pitch `d`). `filt` is what the wgmma filter
 // streams through TMA: bf16 (pitch multiple of 8 elements) for a bf16 index, fp32 (pitch multiple of 4)
 // read as TF32 for an fp32 index; it aliases `store` whenever the pitch already qualifies.
 struct MatView {
@@ -88,10 +88,10 @@ struct MatView {
     int64_t n = 0;
     int32_t d = 0;
     int32_t dtype = B2_F32;       // element type of `store`
-    int32_t filt_dtype = B2_F32;  // element type of `filt`: B2_BF16 -> kind::f16 MMA, B2_F32 -> kind::tf32 MMA
+    int32_t filt_dtype = B2_F32;  // element type of `filt`: B2_BF16 -> bf16 wgmma, B2_F32 -> tf32 wgmma
     int64_t filt_pitch = 0;  // elements
     // fp32 stores only (optional): a bf16 rounding of the rows, pitch multiple of 8. When present, searches run a FIRST level on it
-    // (kind::f16 at twice the tf32 rate, operand error 2^-8 per fp32 operand in the certificate) and only the queries whose
+    // (bf16 wgmma at twice the tf32 rate, operand error 2^-8 per fp32 operand in the certificate) and only the queries whose
     // certificate fails there go through the tf32 filter on `filt`.
     const void* filt16 = nullptr;
     int64_t filt16_pitch = 0;
@@ -103,7 +103,7 @@ struct MatView {
 struct SearchWorkspace;
 
 // ---- kernels / launchers (one per .cu) ------------------------------------------------------------------
-// knn_filter_sm100.cu
+// knn_filter_sm90.cu
 int filter_kp_for_k(int k);  // candidate-list capacity used for a given k, 0 = k too large for the filter
 int launch_knn_filter(const MatView& X, const void* q_filt, int64_t q_pitch, int64_t nq, int metric, int kp,
                       int n_splits, bool two_cta, float* cand_score, int32_t* cand_id, float* cand_thr, int device,

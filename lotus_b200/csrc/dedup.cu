@@ -1,5 +1,5 @@
 // dedup.cu — sem_dedup's data-parallel core (lotus/sem_ops/sem_dedup.py:45-84) without the N x N DataFrame:
-//   b2_threshold_pairs     : tcgen05 all-pairs filter (upper triangle only) -> exact canonical verification of the
+//   b2_threshold_pairs     : wgmma all-pairs filter (upper triangle only) -> exact canonical verification of the
 //                            candidates with the reference's strict `score > threshold` -> pair list sorted by (i, j)
 //   b2_connected_components: lock-free union-find (link larger root under smaller root) + path compression;
 //                            label = smallest row id of the component, the deterministic stand-in for the
@@ -159,7 +159,7 @@ int b2_threshold_pairs(b2_index* idx, float threshold, int32_t part, int32_t npa
     std::vector<int32_t> hi, hj;
     if (found > 0) {
         if ((rc = ver_i.ensure(found * sizeof(int32_t))) != B2_OK || (rc = ver_j.ensure(found * sizeof(int32_t))) != B2_OK) { cleanup(); return rc; }
-        const int64_t blocks = std::min<int64_t>(ceil_div((int64_t)found * 32, 256), 148 * 16);
+        const int64_t blocks = std::min<int64_t>(ceil_div((int64_t)found * 32, 256), 132 * 16);
         pair_verify_kernel<<<(unsigned)blocks, 256, 0, st>>>(reinterpret_cast<const char*>(X.store), X.dtype, X.d, cand_i.as<int32_t>(),
                                                              cand_j.as<int32_t>(), (int64_t)found, threshold, ver_i.as<int32_t>(),
                                                              ver_j.as<int32_t>(), d_cnt + 1);
@@ -214,11 +214,11 @@ int b2_connected_components(int64_t n, const int64_t* pi, const int64_t* pj, int
         cudaMemcpy(dpi.p, pi, n_pairs * sizeof(int64_t), cudaMemcpyHostToDevice);
         cudaMemcpy(dpj.p, pj, n_pairs * sizeof(int64_t), cudaMemcpyHostToDevice);
     }
-    const unsigned gn = (unsigned)std::min<int64_t>(ceil_div(n, 256), 148 * 16);
+    const unsigned gn = (unsigned)std::min<int64_t>(ceil_div(n, 256), 132 * 16);
     uf_init_kernel<<<gn, 256>>>(parent.as<int64_t>(), n);
     g_stats[ST_LAUNCHES]++;
     if (n_pairs) {
-        const unsigned gm = (unsigned)std::min<int64_t>(ceil_div(n_pairs, 256), 148 * 16);
+        const unsigned gm = (unsigned)std::min<int64_t>(ceil_div(n_pairs, 256), 132 * 16);
         uf_union_kernel<<<gm, 256>>>(parent.as<int64_t>(), dpi.as<int64_t>(), dpj.as<int64_t>(), n_pairs, n, reinterpret_cast<int*>(derr.p));
         g_stats[ST_LAUNCHES]++;
     }

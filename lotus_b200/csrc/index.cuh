@@ -113,7 +113,7 @@ static inline size_t esize(int dtype) { return dtype == B2_F32 ? 4 : 2; }
 // searchable view (filter operand, row norms, max norm) of a row-major device matrix
 int build_view(const void* store, int64_t n, int d, int dtype, DevBuf& filt_pad, DevBuf& norm2, DevBuf& scalar, MatView& v,
                cudaStream_t st, DevBuf* filt16 = nullptr);
-// the exact top-k pipeline on device buffers: tcgen05 filter -> finalize/certify -> dense fallback
+// the exact top-k pipeline on device buffers: wgmma filter -> finalize/certify -> dense fallback
 int search_core(b2_index* idx, const MatView& X, int metric, const void* q_dev, int q_dtype, int64_t nq, int k,
                 const int64_t* id_map, int64_t id_offset, float* out_sc, int64_t* out_id, cudaStream_t st, int level = 0);
 float filter_rel_eps(int store_dtype, int filt_dtype, int q_dtype, int d);

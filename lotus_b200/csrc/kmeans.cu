@@ -7,7 +7,7 @@
 //
 // Device pipeline of one Lloyd iteration (everything stays on the device; the only host round trip is one 4-byte counter):
 //   1. centroid view  : bf16 (or tf32) filter copy of the fp32 centroids + canonical squared norms + max norm (device scalar)
-//   2. filter         : knn_filter_kernel<16, L2, ., ., TOP1> — tcgen05 scores of every point against every centroid, the
+//   2. filter         : knn_filter_kernel<16, L2, ., ., TOP1> — wgmma scores of every point against every centroid, the
 //                       epilogue keeps each point's best two centroids and the third-best score in registers
 //   3. km_assign_finalize_kernel (thread per point): winner c1 by filter score, runner-up bound f2 (second best, third-best
 //                       bounds of every list). |filter - exact| <= eps for every centroid, so f1 - f2 > 2 eps (+ fp32 rounding
@@ -675,7 +675,7 @@ int assign_points(b2_index* idx, const void* pts, const float* pnorm2, int64_t m
     const int d = idx->d;
     MatView cv;
     B2_TRY(centroid_view(cent, k, d, idx->dtype, w, cv, st));
-    int dev_sms = 148;
+    int dev_sms = 132;
     cudaDeviceGetAttribute(&dev_sms, cudaDevAttrMultiProcessorCount, idx->device);
     const int filt_dtype = cv.filt_dtype;
     const int kp = 16;
@@ -796,7 +796,7 @@ int update_centroids(b2_index* idx, const void* x, const int64_t* row_ids, int64
     // one warp, whatever the lane width (4 / 8 / 16 B), the ring depth (64 / 256 rows) or the copy mechanism (cp.async / TMA bulk).
     static const int lane_bytes_env = [] { const char* e = getenv("B2_KM_LANE_BYTES"); const int v = e ? atoi(e) : 0; return (v == 4 || v == 16) ? v : 0; }();
     const size_t row_bytes_total = (size_t)d * esize(idx->dtype);
-    int sms = 148;
+    int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, idx->device);
     int LB = lane_bytes_env ? lane_bytes_env : ((int64_t)k * (int64_t)ceil_div((int64_t)row_bytes_total, 512) >= 4LL * 6 * sms ? 16 : 4);
     if (LB == 16 && (row_bytes_total % 16 != 0 || (reinterpret_cast<uintptr_t>(x) % 16) != 0)) LB = 4;
@@ -963,13 +963,13 @@ int kmeans_impl(b2_index* idx, const int64_t* ids_host, int64_t m, int k, int ni
     int cur = 0;
     if (nx == k) {
         // "Number of training points same as number of centroids, just copying"
-        rows_to_f32_kernel<<<148, 256, 0, st>>>(T, idx->dtype, d, nullptr, k, w.cent[0].as<float>());
+        rows_to_f32_kernel<<<132, 256, 0, st>>>(T, idx->dtype, d, nullptr, k, w.cent[0].as<float>());
         B2_LAUNCH_CHECK();
     } else {
         rand_perm_prefix(perm, nx, k, seed + 1);
         B2_TRY(w.perm.ensure((size_t)k * sizeof(int64_t)));
         B2_CUDA(cudaMemcpyAsync(w.perm.p, perm.data(), (size_t)k * sizeof(int64_t), cudaMemcpyHostToDevice, st));
-        rows_to_f32_kernel<<<148, 256, 0, st>>>(T, idx->dtype, d, w.perm.as<int64_t>(), k, w.cent[0].as<float>());
+        rows_to_f32_kernel<<<132, 256, 0, st>>>(T, idx->dtype, d, w.perm.as<int64_t>(), k, w.cent[0].as<float>());
         B2_LAUNCH_CHECK();
         B2_CUDA(cudaStreamSynchronize(st));
         B2_TRY(w.assign.ensure((size_t)nx * sizeof(int64_t)));

@@ -1,6 +1,6 @@
 // knn_exact.cu — the exact side of the search pipeline (everything that decides the reported result).
 //
-//   finalize_kernel   : per query (one warp): merge the per-split candidate lists of the tcgen05 filter with a
+//   finalize_kernel   : per query (one warp): merge the per-split candidate lists of the wgmma filter with a
 //                       warp-shuffle bitonic network, re-score the KP survivors in the canonical fp64 order,
 //                       sort them, apply faiss's heap tie rule, and CERTIFY the result against everything the
 //                       filter discarded (rigorous error margin). Uncertified queries are flagged.
@@ -878,7 +878,7 @@ __global__ void fill_f32_kernel(float* p, int64_t n, float v) {
     for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < n; t += (int64_t)gridDim.x * blockDim.x) p[t] = v;
 }
 
-int grid_for(int64_t work_items, int threads, int cap = 148 * 16) {
+int grid_for(int64_t work_items, int threads, int cap = 132 * 16) {
     int64_t g = ceil_div(work_items, threads);
     if (g < 1) g = 1;
     return (int)std::min<int64_t>(g, cap);
@@ -933,7 +933,7 @@ int launch_exact_l2_assigned(const void* pts, int dtype, int64_t m, int d, const
         return B2_ERANGE;
     }
     if (smem > 48 * 1024) B2_CUDA(cudaFuncSetAttribute(exact_l2_assigned_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    exact_l2_assigned_kernel<<<grid_for(m * 32, 256, 148 * 8), 256, smem, stream>>>(pts, dtype, m, d, cent, assign, out);
+    exact_l2_assigned_kernel<<<grid_for(m * 32, 256, 132 * 8), 256, smem, stream>>>(pts, dtype, m, d, cent, assign, out);
     B2_LAUNCH_CHECK();
     return B2_OK;
 }
@@ -1057,7 +1057,7 @@ int launch_dense_topk(const MatView& X, const void* q, int q_dtype, int64_t nq, 
         // without a selection list the batch is the contiguous query range [s0, s0+sc)
         const void* qb = q_sel ? q : reinterpret_cast<const char*>(q) + (size_t)s0 * X.d * (q_dtype == B2_F32 ? 4 : 2);
         if (X.n > 0) {
-            dense_scores_kernel<<<grid_for(X.n * 32, 256, 148 * 8), 256, smem, stream>>>(X.store, X.dtype, X.n, X.d, qb, q_dtype,
+            dense_scores_kernel<<<grid_for(X.n * 32, 256, 132 * 8), 256, smem, stream>>>(X.store, X.dtype, X.n, X.d, qb, q_dtype,
                                                                                        sel, sc, metric, dense_ws);
             B2_LAUNCH_CHECK();
         }

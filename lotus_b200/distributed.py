@@ -1,6 +1,6 @@
 """Row-sharded flat index across the GPUs of one box (SURVEY §8e): one process per GPU, torch.distributed for the
 plumbing. The corpus rows [r*N/G, (r+1)*N/G) live on rank r; queries are replicated; every rank runs the fused
-tcgen05 filter + exact finalize on its shard, then ONE all-gather of the per-shard (score, idx) lists over
+wgmma filter + exact finalize on its shard, then ONE all-gather of the per-shard (score, idx) lists over
 NCCL/NVLink and a single-kernel k-way merge (b2_merge_topk_dev). No other collective touches the data path.
 
 The reference is single-process (faiss_vs.py); the sharded result is defined as faiss `IndexShards` would define
@@ -192,7 +192,7 @@ def merge_host_lists(scores: np.ndarray, idx: np.ndarray, metric: int):
 # ---- multi-GPU dedup and k-means (SURVEY.md §8e) ----------------------------------------------------------------------
 def sharded_threshold_pairs(index: "nv.Index", threshold: float, group=None):
     """All pairs i<j with score > threshold when EVERY rank holds the full corpus in `index` (it fits: 7.7 GB for
-    10M x 384 bf16): the upper-triangular tile grid is dealt to the ranks in groups of 148 query tiles (`part`/`nparts` of
+    10M x 384 bf16): the upper-triangular tile grid is dealt to the ranks in groups of one query tile per SM (132 on H100) (`part`/`nparts` of
     b2_threshold_pairs), each rank filters + verifies its tiles, then one all-gather of the sparse pair lists.
     Returns the same (pi, pj) — sorted by (i, j) — on every rank."""
     import torch

@@ -1,6 +1,6 @@
 """`cluster(col_name, ncentroids)` — lotus/utils.py:14-72: returns the function that k-means-clusters a frame's
 indexed column and yields one cluster id per row. The reference calls faiss.Kmeans(d, k, niter, verbose).train(x)
-then kmeans.index.search(x, 1) (:61-65); here both run on the B200 through `vs.kmeans`."""
+then kmeans.index.search(x, 1) (:61-65); here both run on the GPU through `vs.kmeans`."""
 from __future__ import annotations
 
 from typing import Callable

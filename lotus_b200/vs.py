@@ -3,7 +3,7 @@ drop-in replacement of `FaissVS` (lotus/vector_store/faiss_vs.py:13-77) backed b
 
     lotus.settings.configure(rm=rm, vs=B200VS())          # where the reference says vs=FaissVS()
 
-There is no CPU path: without the CUDA library / a B200 every method that computes raises.
+There is no CPU path: without the CUDA library / an H100 every method that computes raises.
 """
 from __future__ import annotations
 
@@ -112,7 +112,7 @@ def _to_host_matrix(a: Any, want_bf16: bool, exact_bf16_ok: bool = False, scratc
 
 
 class MultiDeviceIndex:
-    """Row-sharded flat index over several B200s driven from ONE process (for users who do not run under torchrun; under
+    """Row-sharded flat index over several H100s driven from ONE process (for users who do not run under torchrun; under
     torchrun use lotus_b200.distributed.ShardedIndex, whose exchange runs over NCCL/NVLink). Shard g holds the contiguous rows
     `shard_bounds(n, G, g)` on devices[g]; a search runs the G per-device C-ABI calls concurrently (ctypes releases the GIL),
     then merges the G sorted lists on the host with the same (score, shard order) rule as the k-way merge kernel.
@@ -192,7 +192,7 @@ def merge_shard_lists(D_parts: list, I_parts: list, metric: int):
 
 
 class B200VS(VS):
-    """Flat (brute-force, exact) vector store on one B200 (or, with devices=[...], row-sharded over several from one process).
+    """Flat (brute-force, exact) vector store on one H100 (or, with devices=[...], row-sharded over several from one process).
 
     Args mirror FaissVS(factory_string="Flat", metric=faiss.METRIC_INNER_PRODUCT) (faiss_vs.py:14).
     dtype: "f32" (store what faiss would: float32), "bf16" (round the corpus to bfloat16 once; exact search

@@ -2,7 +2,7 @@
 
 CPU restatement of the faiss-cpu 1.13 algorithms behind the reference's hot path
 (lotus/vector_store/faiss_vs.py:22-77, lotus/utils.py:61-65). PARITY UNPINNED: faiss itself is
-not available in this image (nor on the GPU box) and the reference holds no golden vectors for this
+not installed where this project is built and tested and the reference holds no golden vectors for this
 path, so the restatement is pinned only against hand-derived known answers (tests/golden/) and
 independent numpy cross-checks. bench.py `faiss_probe()` / `cpu_arms()` switch to the real wheel the
 day `import faiss` succeeds and print the comparison with this restatement.
@@ -33,7 +33,7 @@ CANONICAL, F32_SEQ, F32_FAST = 0, 1, 2
 
 
 def build(force: bool = False) -> str:
-    """gcc-compile oracle/faiss_flat.c into oracle/liborc.so (git-ignored, travels with gpurun)."""
+    """gcc-compile oracle/faiss_flat.c into oracle/liborc.so (git-ignored build product)."""
     if not force and os.path.exists(_LIB) and os.path.getmtime(_LIB) >= os.path.getmtime(_SRC):
         return _LIB
     cmd = ["gcc", "-O3", "-march=x86-64-v3", "-ffp-contract=off", "-fopenmp", "-fPIC", "-shared",
@@ -51,9 +51,34 @@ _native_lib = None
 _native_flags = None
 
 
+def _owned_by_me(path: str) -> bool:
+    """path exists, belongs to this user and is writable by nobody else."""
+    try:
+        st = os.stat(path)
+    except OSError:
+        return False
+    return st.st_uid == os.getuid() and not (st.st_mode & 0o022)
+
+
+def _private_build_dir() -> str:
+    """$XDG_CACHE_HOME/lotus_b200 or ~/.cache/lotus_b200 when it is this user's and private, else a fresh mkdtemp."""
+    import tempfile
+    for base in (os.environ.get("XDG_CACHE_HOME"), os.path.join(os.path.expanduser("~"), ".cache")):
+        if not base:
+            continue
+        d = os.path.join(base, "lotus_b200")
+        try:
+            os.makedirs(d, mode=0o700, exist_ok=True)
+        except OSError:
+            continue
+        if _owned_by_me(d):
+            return d
+    return tempfile.mkdtemp(prefix="lotus_b200_")
+
+
 def native_lib():
     """The same source compiled ON THIS HOST with -march=native (AVX-512 where the host has it) and fp contraction, for the TIMED
-    CPU arm only (bench.py): the portable liborc.so is built in the build container for x86-64-v3 so that it runs anywhere and
+    CPU arm only (bench.py): the portable liborc.so is built by build() for x86-64-v3 so that it runs anywhere and
     keeps -ffp-contract=off for the canonical scorer. Falls back to the portable library when gcc is not available here."""
     global _native_lib, _native_flags
     if _native_lib is not None:
@@ -71,9 +96,14 @@ def native_lib():
         except OSError:
             pass
         tag = hashlib.sha1((cpu + open(_SRC).read()).encode()).hexdigest()[:12]
-        path = os.path.join(_HERE, f"liborc_native_{tag}.so")
-        if not os.path.exists(path):
-            subprocess.run(["gcc", *flags, "-fopenmp", "-fPIC", "-shared", "-o", path, _SRC, "-lm"], check=True, capture_output=True, text=True)
+        # compiled at run time, so it goes to a directory of this user's (the source tree may be read-only, and a shared
+        # temporary directory would let another user plant the library)
+        path = os.path.join(_private_build_dir(), f"liborc_native_{tag}.so")
+        if not _owned_by_me(path):
+            tmp = f"{path}.{os.getpid()}"
+            subprocess.run(["gcc", *flags, "-fopenmp", "-fPIC", "-shared", "-o", tmp, _SRC, "-lm"], check=True, capture_output=True, text=True)
+            os.chmod(tmp, 0o755)
+            os.replace(tmp, path)
         L = ctypes.CDLL(path)
         _native_flags = " ".join(flags)
     except Exception:

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (run with -m gpu on a machine with one)")
 
 
 @pytest.fixture(scope="session")
@@ -22,6 +22,6 @@ def nv():
 
 @pytest.fixture(scope="session")
 def gpu(nv):
-    """GPU tests FAIL (not skip) when no B200 is visible: a silent skip would hide a fallback."""
-    assert nv.device_count() >= 1, "no sm_100 device visible: -m gpu tests must run on the B200 box"
+    """GPU tests FAIL (not skip) when no H100 is visible: a silent skip would hide a fallback."""
+    assert nv.device_count() >= 1, "no sm_90 device visible: -m gpu tests must run on an H100"
     return nv

@@ -1,8 +1,8 @@
 """Generates tests/golden/reference_ops.json by running the REFERENCE's own operator code.
 
-    PYTHONHASHSEED=0 python tests/golden/make_reference_golden.py        (needs /root/reference; run in the build container)
+    PYTHONHASHSEED=0 python tests/golden/make_reference_golden.py        (needs a checkout of the reference in LOTUS_REFERENCE)
 
-/root/reference (lotus-data/lotus @ 136ae4f4) is pure Python but cannot be imported as is: litellm, faiss,
+The reference (lotus-data/lotus @ 136ae4f4) is pure Python but cannot be imported as is: litellm, faiss,
 sentence_transformers, backoff, ... are absent from this image. This script
   * satisfies every missing third-party import with an inert mock EXCEPT `faiss`, for which it installs a small stand-in
     module whose IndexFlat / Kmeans / read_index / write_index are backed by the oracle (oracle/faiss_flat.c) and by
@@ -11,7 +11,7 @@ sentence_transformers, backoff, ... are absent from this image. This script
     `sem_dedup`, `sem_cluster_by` (lotus/sem_ops/*.py, lotus/utils.py) on small seeded inputs;
   * stores inputs and resulting DataFrames as JSON.
 tests/test_reference_golden.py (CPU, oracle-backed test double) and tests/test_gpu_ops.py (B200VS) replay the scenarios
-through lotus_b200's accessors and must reproduce the frames. Nothing reads /root/reference at test time.
+through lotus_b200's accessors and must reproduce the frames. Nothing reads the reference at test time.
 """
 import importlib.abc
 import importlib.machinery
@@ -104,7 +104,10 @@ class _Kmeans:
 faiss.index_factory, faiss.write_index, faiss.read_index, faiss.Kmeans = _index_factory, _write_index, _read_index, _Kmeans
 sys.modules["faiss"] = faiss
 sys.meta_path.append(_MockFinder())
-sys.path.insert(0, "/root/reference")
+REF = os.environ.get("LOTUS_REFERENCE")
+if not REF or not os.path.isdir(os.path.join(REF, "lotus")):
+    sys.exit("set LOTUS_REFERENCE to a checkout of lotus-data/lotus @ 136ae4f4 (the directory that holds lotus/)")
+sys.path.insert(0, REF)
 import lotus  # noqa: E402  (the REFERENCE package)
 from lotus.models import RM  # noqa: E402
 from lotus.vector_store import FaissVS  # noqa: E402

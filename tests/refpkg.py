@@ -1,7 +1,7 @@
 """Imports the UNMODIFIED reference package (lotus-data/lotus) for tests and for bench.py's operator-scope reference leg.
 
-The package lives under baseline/_ref (scripts/install_reference.py; git-ignored, shipped to the GPU box by gpurun) — in the
-build container /root/reference is used when baseline/_ref is absent. Its third-party imports that this image lacks (litellm,
+The package is the build product oracle/_ref/lotus (oracle/reference.py, made by build()); a checkout named by LOTUS_REFERENCE
+is used when that is absent, and without either the callers report the reference as unavailable. Its third-party imports that this image lacks (litellm,
 sentence_transformers, backoff, ...) are satisfied by inert mocks: none of them is on the embedding-similarity path. `faiss` is
 either the real wheel (if importable), a stand-in handed in by the caller (bench: oracle-backed, to time the reference's
 operator code around it), or an inert mock (drop-in test: B200VS replaces FaissVS, nothing may call faiss).
@@ -40,8 +40,8 @@ class _MockFinder(importlib.abc.MetaPathFinder, importlib.abc.Loader):
 
 
 def reference_dir() -> str | None:
-    for cand in (os.path.join(ROOT, "baseline", "_ref"), "/root/reference"):
-        if os.path.isfile(os.path.join(cand, "lotus", "__init__.py")):
+    for cand in (os.path.join(ROOT, "oracle", "_ref"), os.environ.get("LOTUS_REFERENCE")):
+        if cand and os.path.isfile(os.path.join(cand, "lotus", "__init__.py")):
             return cand
     return None
 
@@ -50,7 +50,7 @@ def import_reference(faiss_module=None):
     """-> (lotus module, description of what stands for faiss) or (None, reason)."""
     where = reference_dir()
     if where is None:
-        return None, "reference package not found (run scripts/install_reference.py in the build container)"
+        return None, "reference package not found (build() puts it under oracle/_ref from a checkout named by LOTUS_REFERENCE)"
     mock = list(MISSING)
     faiss_kind = "real faiss wheel"
     if faiss_module is not None:

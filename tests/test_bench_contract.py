@@ -38,7 +38,7 @@ def test_reference_arm_sizes_its_own_sample():
     assert r.returncode == 0, r.stderr[-2000:]
     d = json.loads(r.stdout.strip().splitlines()[-1])
     assert 128 <= d["reference_run"]["sample_queries_per_step"] <= 300 and d["value"] > 0
-    assert set(d["config"]) == {"workload", "nq", "n", "d", "k", "parallelism", "l2_policy"}  # the B200 arm's config keys
+    assert set(d["config"]) == {"workload", "nq", "n", "d", "k", "parallelism", "l2_policy"}  # the GPU arm's config keys
 
 
 def test_reference_arm_uses_every_core_even_under_torchrun_env():

@@ -1,4 +1,4 @@
-"""The pandas operators end to end on the B200 (B200VS through the C-ABI) against oracle-derived expectations, plus
+"""The pandas operators end to end on the H100 (B200VS through the C-ABI) against oracle-derived expectations, plus
 the dedup / k-means / merge entry points."""
 import os
 

@@ -1,5 +1,5 @@
-"""sem_dedup's all-pairs kernel in both CTA modes — cta_group::2 pairs (the default since round 2: 1370 vs 1250 TFLOP/s at
-10M rows) and single CTAs (B2_PAIR_2CTA=0). The switch is read once per process -> subprocess, bounded by a timeout because
+"""sem_dedup's all-pairs kernel in both CTA modes — CTA pairs sharing each corpus tile through TMA multicast (the default)
+and single CTAs (B2_PAIR_2CTA=0). The switch is read once per process -> subprocess, bounded by a timeout because
 a barrier-protocol mistake would hang. Identical pair lists to the oracle, whole and sharded."""
 import json
 import os

@@ -42,7 +42,7 @@ def check(nv, x, q, k, metric, dtype, ids=None, expect_filter=None):
     assert np.array_equal(I, Io), f"top-k indices differ in {(I != Io).any(axis=1).sum()} of {len(I)} rows"
     assert np.array_equal(bits(D), bits(Do)), "scores are not bit-identical to the canonical oracle score"
     if expect_filter is True:
-        assert st["filter_launches"] >= 1, "the tcgen05 filter did not run"
+        assert st["filter_launches"] >= 1, "the wgmma filter did not run"
     if expect_filter is False:
         assert st["filter_launches"] == 0
     return st

@@ -364,7 +364,7 @@ def test_f32_to_bf16_rounding_matches_the_reference_formula_and_keeps_nan():
 
 
 def test_quickstart_example_runs_against_the_test_double(monkeypatch, capsys):
-    # examples/quickstart.py needs a B200; its control flow (all five operators) is exercised here with the oracle-backed VS
+    # examples/quickstart.py needs an H100; its control flow (all five operators) is exercised here with the oracle-backed VS
     import lotus_b200.sem_ops.sem_dedup as sd
     monkeypatch.setattr(sd.nv, "connected_components", lambda n, pi, pj, device=0: oracle.connected_components(n, pi, pj))
     path = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "examples", "quickstart.py")
@@ -450,7 +450,7 @@ def test_sem_search_k_doubling_branch_equals_the_ids_branch_and_rerank_reorders(
 
 
 def _schedule_items(plan, nq, n, workers):
-    """Python mirror of knn_filter_sm100.cu item_range / num_items (non-pair mode): -> per worker the list of (unit, split, t0, t1)."""
+    """Python mirror of knn_filter_sm90.cu item_range / num_items (non-pair mode): -> per worker the list of (unit, split, t0, t1)."""
     n_mtiles = -(-nq // 128)
     n_units = -(-n_mtiles // 2) if plan["two_cta"] else n_mtiles
     n_ntiles = -(-n // 256)
@@ -479,7 +479,7 @@ def test_filter_schedule_covers_every_unit_tile_pair_once(nq, n, k):
     from lotus_b200 import _native as nv
     plan = nv.filter_plan(nq, n, k)
     assert plan["kp"] > 0 and plan["n_splits"] >= 1
-    workers = 74 if plan["two_cta"] else 148
+    workers = 66 if plan["two_cta"] else 132
     per_worker, n_units, n_ntiles = _schedule_items(plan, nq, n, workers)
     assert plan["units_whole"] % workers == 0 and 0 <= plan["units_whole"] <= n_units
     cover = np.zeros((n_units, n_ntiles), dtype=np.int32)

@@ -1,5 +1,5 @@
-"""CPU dry run of the drop-in worker (tests/ref_dropin_worker.py): the REAL reference package (baseline/_ref, or /root/reference
-in the build container) + lotus_b200.install() + the reference's unmodified operator classes over B200VS, with the native index
+"""CPU dry run of the drop-in worker (tests/ref_dropin_worker.py): the REAL reference package (oracle/_ref, made by
+build()) + lotus_b200.install() + the reference's unmodified operator classes over B200VS, with the native index
 replaced by the oracle-backed fake. Checks the plumbing the GPU test relies on; the numbers come from the oracle here."""
 import json
 import os
@@ -15,7 +15,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 
 def test_reference_operators_over_b200vs_plumbing():
     if refpkg.reference_dir() is None:
-        pytest.skip("reference package not present (scripts/install_reference.py puts it under baseline/_ref)")
+        pytest.skip("reference package not present (build() puts it under oracle/_ref)")
     r = subprocess.run([sys.executable, os.path.join(HERE, "ref_dropin_worker.py")], capture_output=True, text=True, timeout=600,
                        env=dict(os.environ, B2_TEST_FAKE_NATIVE="1"))
     assert r.returncode == 0, r.stderr[-3000:]
