@@ -109,42 +109,143 @@ __global__ void fill_pad_kernel(float* sc, int64_t* id, int64_t total, float pad
     }
 }
 
-// level 0: the caller's search. For an fp32 store with a bf16 copy (X.filt16) and a small k it is the FIRST level of a two-level
-// search: bf16 filter with a longer candidate list, the queries whose certificate fails are deferred, gathered and answered by
-// a level-1 call (tf32 filter on the same store, then the dense path for what still fails) and scattered back.
+// The filter run of a search: for an fp32 store with a bf16 copy (X.filt16) and a small k it is the FIRST level of a two-level
+// search (bf16 filter, longer candidate list). Every caller filters exactly as planned here; b2_debug_filter_plan reports it.
+int plan_filter(const MatView& X_in, const void* q, int q_dtype, int64_t nq, int k, bool top1, int num_sms, FilterPlan& p) {
+    p = FilterPlan();
+    p.q = q;
+    p.q_dtype = q_dtype;
+    p.nq = nq;
+    p.k = k;
+    p.top1 = top1;
+    p.X = X_in;
+    // candidate capacity of the bf16 first level (the 2^-8 operand error lets more rows straddle the k-th score): 0 = not used
+    const int kp16 = (X_in.filt16 && X_in.n >= 4096) ? (k <= 4 ? 32 : k <= 12 ? 64 : k <= 24 ? 72 : 0) : 0;
+    p.two_level = kp16 != 0;
+    if (p.two_level) {
+        p.X.filt = X_in.filt16;
+        p.X.filt_pitch = X_in.filt16_pitch;
+        p.X.filt_dtype = B2_BF16;
+    }
+    const MatView& X = p.X;
+    p.kp = p.two_level ? kp16 : filter_kp_for_k(k);
+    p.min_splits = filter_min_splits_for_k(k);
+    // the filter needs a corpus worth tiling: two tiles at least, and for k > 40 enough tiles to cut into min_splits splits
+    // with k well below the rows of a split. The k-means assignment has no other path.
+    p.use_filter = top1 || (p.kp != 0 && X.n >= 512 && ceil_div(X.n, 256) >= p.min_splits && X.n >= 4 * (int64_t)k);
+    if (!p.use_filter) return B2_OK;
+    p.q_pitch = round_up(X.d, X.filt_dtype == B2_F32 ? 4 : 8);
+    p.q_in_place = q_dtype == X.filt_dtype && p.q_pitch == X.d && (reinterpret_cast<uintptr_t>(q) & 15) == 0;
+    p.rel_eps = filter_rel_eps(X.dtype, X.filt_dtype, q_dtype, X.d);
+    // bound the candidate workspace (nqc x n_splits x kp x 8 bytes) to a few GB: fewer queries per chunk when k needs many splits
+    p.chunk = top1 ? (int64_t)1 << 23
+                   : std::max<int64_t>(4096, std::min<int64_t>(1 << 20, (4LL << 30) / ((int64_t)std::max(p.min_splits, 8) * p.kp * 8)));
+    for (int64_t q0 = 0; q0 < nq; q0 += p.chunk) {
+        FilterChunk c;
+        c.q0 = q0;
+        c.nq = std::min<int64_t>(p.chunk, nq - q0);
+        c.two_cta = filter_use_pair(c.nq);
+        // the k-means top-2 epilogue keeps the uniform split schedule
+        c.n_splits = filter_choose_splits(c.nq, X.n, num_sms, c.two_cta, top1, p.min_splits, top1 ? nullptr : &c.units_whole);
+        if (c.n_splits <= 0) {
+            set_error("internal: no valid corpus split for k=%d over %lld rows", k, (long long)X.n);
+            return B2_EINVAL;
+        }
+        p.chunks.push_back(c);
+    }
+    return B2_OK;
+}
+
+int run_filter(b2_index* idx, const FilterPlan& p, const FilterChunk& c, int metric, cudaStream_t st) {
+    const MatView& X = p.X;
+    const void* q_filt = reinterpret_cast<const char*>(p.q) + (size_t)c.q0 * X.d * esize(p.q_dtype);
+    if (!p.q_in_place) {
+        B2_TRY(idx->q_filt.ensure((size_t)c.nq * p.q_pitch * esize(X.filt_dtype)));
+        B2_TRY(launch_prep_queries(q_filt, p.q_dtype, c.nq, X.d, idx->q_filt.p, X.filt_dtype, p.q_pitch, st));
+        q_filt = idx->q_filt.p;
+    }
+    B2_TRY(idx->cand_score.ensure((size_t)c.nq * c.n_splits * p.kp * sizeof(float)));
+    B2_TRY(idx->cand_id.ensure((size_t)c.nq * c.n_splits * p.kp * sizeof(int32_t)));
+    B2_TRY(idx->cand_thr.ensure((size_t)c.nq * c.n_splits * 2 * sizeof(float)));  // two epilogue sets per split
+    B2_CUDA(cudaEventRecord(idx->ev0, st));
+    B2_TRY(launch_knn_filter(X, q_filt, p.q_pitch, c.nq, metric, p.kp, c.n_splits, c.two_cta, idx->cand_score.as<float>(),
+                             idx->cand_id.as<int32_t>(), idx->cand_thr.as<float>(), idx->device, st, p.top1, c.units_whole));
+    B2_CUDA(cudaEventRecord(idx->ev1, st));
+    return B2_OK;
+}
+
+// rows of the dense path's score workspace (score row of 4 bytes per column, plus two sort-key buffers on the full-sort path)
+// within 512 MB
+static int64_t dense_rows_cap(int64_t n, bool full_sort) {
+    return std::max<int64_t>(1, (int64_t)(512ull << 20) / (std::max<int64_t>(n, 1) * (full_sort ? 24 : 4)));
+}
+
+// Finalize/certify the candidate lists run_filter left for chunk c (hint: a lower bound the k-th score is known to reach, or
+// null), read the one counter back and add the filter's event time to idx->last_filter_ms. The queries the certificate leaves
+// open are compacted into idx->sel[1 .. 1 + *n_open]; with `fallback` the exact dense path answers them here.
+static int certify(b2_index* idx, const FilterPlan& p, const FilterChunk& c, int metric, const int64_t* id_map, int64_t id_offset,
+                   float* out_sc, int64_t* out_id, const float* hint, bool fallback, int64_t* n_open, cudaStream_t st) {
+    const MatView& X = p.X;
+    const void* qc = reinterpret_cast<const char*>(p.q) + (size_t)c.q0 * X.d * esize(p.q_dtype);
+    float* osc = out_sc + (size_t)c.q0 * p.k;
+    int64_t* oid = out_id + (size_t)c.q0 * p.k;
+    B2_TRY(idx->flags.ensure((size_t)c.nq * sizeof(int32_t)));
+    B2_TRY(idx->sel.ensure((size_t)(c.nq + 1) * sizeof(int32_t)));  // [0] = counter, [1..] = uncertified queries
+    B2_TRY(idx->h_flags.ensure(64));
+    int32_t* sel_count = idx->sel.as<int32_t>();
+    int32_t* sel_list = sel_count + 1;
+    B2_CUDA(cudaMemsetAsync(sel_count, 0, sizeof(int32_t), st));
+    B2_TRY(launch_finalize(X, qc, p.q_dtype, c.nq, metric, p.k, p.kp, p.kp / 2, 2 * c.n_splits, idx->cand_score.as<float>(),
+                           idx->cand_id.as<int32_t>(), idx->cand_thr.as<float>(), p.rel_eps, id_map, id_offset, osc, oid,
+                           idx->flags.as<int32_t>(), sel_list, sel_count, st, hint));
+    // the certificate outcome comes back as ONE counter (the failed queries are compacted on the device)
+    int32_t* h_count = reinterpret_cast<int32_t*>(idx->h_flags.p);
+    B2_CUDA(cudaMemcpyAsync(h_count, sel_count, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    cudaError_t se = cudaStreamSynchronize(st);
+    if (se != cudaSuccess) {
+        set_error("search pipeline failed on the device: %s", cudaGetErrorString(se));
+        return B2_ECUDA;
+    }
+    float ms = -1.f;
+    if (cudaEventElapsedTime(&ms, idx->ev0, idx->ev1) == cudaSuccess)
+        idx->last_filter_ms = (idx->last_filter_ms < 0 ? 0.f : idx->last_filter_ms) + ms;
+    const int64_t n_sel = *h_count;
+    *n_open = n_sel;
+    if (!fallback || n_sel == 0) return B2_OK;
+    // exact fallback for the queries the certificate could not cover
+    if (p.k > dense_max_k()) {
+        set_error("internal: fallback with k=%d", p.k);
+        return B2_ERANGE;
+    }
+    g_stats[ST_FALLBACK] += n_sel;
+    const int64_t rows = std::min<int64_t>(dense_rows_cap(X.n, false), n_sel);
+    B2_TRY(idx->dense.ensure((size_t)rows * X.n * sizeof(float)));
+    return launch_dense_topk(X, qc, p.q_dtype, c.nq, sel_list, n_sel, metric, p.k, id_map, id_offset, idx->dense.as<float>(), rows,
+                             nullptr, osc, oid, st);
+}
+
+// level 0: the caller's search. On a two-level plan the queries whose first-level certificate fails are deferred, gathered and
+// answered by a level-1 call (tf32 filter on the same store, then the dense path for what still fails) and scattered back.
 int search_core(b2_index* idx, const MatView& X_in, int metric, const void* q_dev, int q_dtype, int64_t nq, int k,
                        const int64_t* id_map, int64_t id_offset, float* out_sc, int64_t* out_id, cudaStream_t st, int level) {
     if (level == 0) idx->last_filter_ms = -1.f;
     if (nq <= 0) return B2_OK;
     if (level == 0) g_stats[ST_QUERIES] += nq;
-    // candidate capacity of the bf16 first level (the 2^-8 operand error lets more rows straddle the k-th score): 0 = not used
-    const int kp16 = (X_in.filt16 && level == 0 && X_in.n >= 4096) ? (k <= 4 ? 32 : k <= 12 ? 64 : k <= 24 ? 72 : 0) : 0;
-    MatView X = X_in;
-    if (kp16) {
-        X.filt = X_in.filt16;
-        X.filt_pitch = X_in.filt16_pitch;
-        X.filt_dtype = B2_BF16;
-    }
-    const bool defer = kp16 != 0;
-    int64_t n_deferred = 0;
-    if (X.n <= 0) {
+    if (X_in.n <= 0) {
         fill_pad_kernel<<<132, 256, 0, st>>>(out_sc, out_id, nq * k, metric == B2_METRIC_L2 ? FLT_MAX : -FLT_MAX);
         B2_LAUNCH_CHECK();
         return B2_OK;
     }
-    const int kp = kp16 ? kp16 : filter_kp_for_k(k);
-    const int min_splits = filter_min_splits_for_k(k);
-    // the filter needs a corpus worth tiling: two tiles at least, and for k > 64 enough tiles to cut into min_splits splits
-    // with k well below the rows of a split
-    const bool use_filter = kp != 0 && X.n >= 512 && ceil_div(X.n, 256) >= min_splits && X.n >= 4 * (int64_t)k;
-    const bool full_sort = k > dense_select_max_k();  // dense path sorts whole rows: score + two key buffers per column
-    const int64_t dense_rows_cap = std::max<int64_t>(1, (int64_t)(512ull << 20) / (std::max<int64_t>(X.n, 1) * (full_sort ? 24 : 4)));
-    if (!use_filter) {
+    FilterPlan p;
+    B2_TRY(plan_filter(X_in, q_dev, q_dtype, nq, k, false, sm_count(idx->device), p));
+    const MatView& X = p.X;
+    if (!p.use_filter) {
         if (k > dense_max_k()) {
             set_error("k=%d is not supported (max %d)", k, dense_max_k());
             return B2_ERANGE;
         }
-        const int64_t rows = std::min<int64_t>(dense_rows_cap, nq);
+        const bool full_sort = k > dense_select_max_k();  // dense path sorts whole rows: score + two key buffers per column
+        const int64_t rows = std::min<int64_t>(dense_rows_cap(X.n, full_sort), nq);
         B2_TRY(idx->dense.ensure((size_t)rows * X.n * sizeof(float)));
         if (full_sort) B2_TRY(idx->sort_keys.ensure(dense_sort_ws_bytes(rows, X.n)));
         B2_TRY(launch_dense_topk(X, q_dev, q_dtype, nq, nullptr, nq, metric, k, id_map, id_offset, idx->dense.as<float>(), rows,
@@ -152,75 +253,17 @@ int search_core(b2_index* idx, const MatView& X_in, int metric, const void* q_de
         g_stats[ST_FALLBACK] += nq;
         return B2_OK;
     }
-    int dev_sms = 132;
-    cudaDeviceGetAttribute(&dev_sms, cudaDevAttrMultiProcessorCount, idx->device);
-    const int filt_dtype = X.filt_dtype;
-    const int64_t q_pitch = round_up(X.d, filt_dtype == B2_F32 ? 4 : 8);
-    const float rel_eps = filter_rel_eps(X.dtype, filt_dtype, q_dtype, X.d);
-    // queries that already have the filter's element type and a TMA-compatible pitch are streamed in place
-    const bool q_in_place = q_dtype == filt_dtype && q_pitch == X.d && (reinterpret_cast<uintptr_t>(q_dev) & 15) == 0;
-    // bound the candidate workspace: process the queries in chunks
-    // bound the candidate workspace (nqc x n_splits x kp x 8 bytes) to a few GB: fewer queries per chunk when k needs many splits
-    const int64_t chunk = std::max<int64_t>(4096, std::min<int64_t>(1 << 20, (4LL << 30) / ((int64_t)std::max(min_splits, 8) * kp * 8)));
-    for (int64_t q0 = 0; q0 < nq; q0 += chunk) {
-        const int64_t nqc = std::min<int64_t>(chunk, nq - q0);
-        const char* qc = reinterpret_cast<const char*>(q_dev) + (size_t)q0 * X.d * esize(q_dtype);
-        float* osc = out_sc + (size_t)q0 * k;
-        int64_t* oid = out_id + (size_t)q0 * k;
-        const bool two_cta = filter_use_pair(nqc);
-        int units_whole = 0;
-        const int n_splits = filter_choose_splits(nqc, X.n, dev_sms, two_cta, false, min_splits, &units_whole);
-        if (n_splits <= 0) {
-            set_error("internal: no valid corpus split for k=%d over %lld rows", k, (long long)X.n);
-            return B2_EINVAL;
-        }
-        if (!q_in_place) B2_TRY(idx->q_filt.ensure((size_t)nqc * q_pitch * esize(filt_dtype)));
-        const void* q_filt = q_in_place ? static_cast<const void*>(qc) : idx->q_filt.p;
-        B2_TRY(idx->cand_score.ensure((size_t)nqc * n_splits * kp * sizeof(float)));
-        B2_TRY(idx->cand_id.ensure((size_t)nqc * n_splits * kp * sizeof(int32_t)));
-        B2_TRY(idx->cand_thr.ensure((size_t)nqc * n_splits * 2 * sizeof(float)));  // two epilogue sets per split
-        B2_TRY(idx->flags.ensure((size_t)nqc * sizeof(int32_t)));
-        B2_TRY(idx->sel.ensure((size_t)(nqc + 1) * sizeof(int32_t)));  // [0] = counter, [1..] = uncertified queries
-        B2_TRY(idx->h_flags.ensure(64));
-        int32_t* sel_count = idx->sel.as<int32_t>();
-        int32_t* sel_list = sel_count + 1;
-        B2_CUDA(cudaMemsetAsync(sel_count, 0, sizeof(int32_t), st));
-        if (!q_in_place) B2_TRY(launch_prep_queries(qc, q_dtype, nqc, X.d, idx->q_filt.p, filt_dtype, q_pitch, st));
-        B2_CUDA(cudaEventRecord(idx->ev0, st));
-        B2_TRY(launch_knn_filter(X, q_filt, q_pitch, nqc, metric, kp, n_splits, two_cta, idx->cand_score.as<float>(),
-                                 idx->cand_id.as<int32_t>(), idx->cand_thr.as<float>(), idx->device, st, false, units_whole));
-        B2_CUDA(cudaEventRecord(idx->ev1, st));
-        B2_TRY(launch_finalize(X, qc, q_dtype, nqc, metric, k, kp, kp / 2, 2 * n_splits, idx->cand_score.as<float>(),
-                               idx->cand_id.as<int32_t>(), idx->cand_thr.as<float>(), rel_eps, id_map, id_offset, osc, oid,
-                               idx->flags.as<int32_t>(), sel_list, sel_count, st));
-        // the certificate outcome comes back as ONE counter (the failed queries are compacted on the device)
-        int32_t* h_count = reinterpret_cast<int32_t*>(idx->h_flags.p);
-        B2_CUDA(cudaMemcpyAsync(h_count, sel_count, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-        cudaError_t se = cudaStreamSynchronize(st);
-        if (se != cudaSuccess) {
-            set_error("search pipeline failed on the device: %s", cudaGetErrorString(se));
-            return B2_ECUDA;
-        }
-        float ms = -1.f;
-        if (cudaEventElapsedTime(&ms, idx->ev0, idx->ev1) == cudaSuccess)
-            idx->last_filter_ms = (idx->last_filter_ms < 0 ? 0.f : idx->last_filter_ms) + ms;
-        // exact fallback for the queries the certificate could not cover
-        const int64_t n_sel = *h_count;
-        if (n_sel > 0 && defer) {
+    int64_t n_deferred = 0;
+    for (const FilterChunk& c : p.chunks) {
+        B2_TRY(run_filter(idx, p, c, metric, st));
+        int64_t n_sel = 0;
+        B2_TRY(certify(idx, p, c, metric, id_map, id_offset, out_sc, out_id, nullptr, /*fallback=*/!p.two_level, &n_sel, st));
+        if (p.two_level && n_sel > 0) {
             B2_TRY(idx->defer.ensure((size_t)nq * sizeof(int64_t)));
-            defer_append_kernel<<<(unsigned)ceil_div(n_sel, 256), 256, 0, st>>>(sel_list, n_sel, q0, idx->defer.as<int64_t>() + n_deferred);
+            defer_append_kernel<<<(unsigned)ceil_div(n_sel, 256), 256, 0, st>>>(idx->sel.as<int32_t>() + 1, n_sel, c.q0,
+                                                                               idx->defer.as<int64_t>() + n_deferred);
             B2_LAUNCH_CHECK();
             n_deferred += n_sel;
-        } else if (n_sel > 0) {
-            if (k > dense_max_k()) {
-                set_error("internal: fallback with k=%d", k);
-                return B2_ERANGE;
-            }
-            g_stats[ST_FALLBACK] += n_sel;
-            const int64_t rows = std::min<int64_t>(dense_rows_cap, n_sel);
-            B2_TRY(idx->dense.ensure((size_t)rows * X.n * sizeof(float)));
-            B2_TRY(launch_dense_topk(X, qc, q_dtype, nqc, sel_list, n_sel, metric, k, id_map, id_offset, idx->dense.as<float>(), rows,
-                                     nullptr, osc, oid, st));
         }
     }
     if (n_deferred > 0) {
@@ -244,24 +287,56 @@ int search_core(b2_index* idx, const MatView& X_in, int metric, const void* q_de
     return B2_OK;
 }
 
-// searchable view for an ids subset (faiss_vs.py:57-64: temporary index over vecs[ids])
-static int build_subset(b2_index* idx, const int64_t* ids_dev, int64_t m, MatView& sub, cudaStream_t st) {
-    B2_TRY(idx->sub_store.ensure((size_t)std::max<int64_t>(m, 1) * idx->d * esize(idx->dtype)));
-    B2_TRY(idx->scalar.ensure(64));
-    int* err = reinterpret_cast<int*>(idx->scalar.as<char>() + 16);
+int gather_rows_checked(const void* x, int dtype, int d, const int64_t* ids, int64_t m, int64_t n, void* out, DevBuf& scalar,
+                        cudaStream_t st) {
+    B2_TRY(scalar.ensure(64));
+    int* err = reinterpret_cast<int*>(scalar.as<char>() + 16);
     B2_CUDA(cudaMemsetAsync(err, 0, sizeof(int), st));
-    B2_TRY(launch_gather_rows(idx->store.p, idx->dtype, idx->d, ids_dev, m, idx->n, idx->sub_store.p, err, st));
+    B2_TRY(launch_gather_rows(x, dtype, d, ids, m, n, out, err, st));
     int herr = 0;
     B2_CUDA(cudaMemcpyAsync(&herr, err, sizeof(int), cudaMemcpyDeviceToHost, st));
     B2_CUDA(cudaStreamSynchronize(st));
     if (herr) {
-        set_error("ids contains a position outside [0, %lld)", (long long)idx->n);
+        set_error("ids contains a position outside [0, %lld)", (long long)n);
         return B2_ERANGE;
     }
+    return B2_OK;
+}
+
+// searchable view for an ids subset (faiss_vs.py:57-64: temporary index over vecs[ids])
+static int build_subset(b2_index* idx, const int64_t* ids_dev, int64_t m, MatView& sub, cudaStream_t st) {
+    B2_TRY(idx->sub_store.ensure((size_t)std::max<int64_t>(m, 1) * idx->d * esize(idx->dtype)));
+    B2_TRY(gather_rows_checked(idx->store.p, idx->dtype, idx->d, ids_dev, m, idx->n, idx->sub_store.p, idx->scalar, st));
     return build_view(idx->sub_store.p, m, idx->d, idx->dtype, idx->sub_filt, idx->sub_norm2, idx->scalar, sub, st, &idx->sub_filt16);
 }
 
+// Runs body(lo, hi) over [0, count) in chunks of 2^20 elements on up to 16 host threads.
+template <typename Body>
+static void for_each_chunk(int64_t count, const Body& body) {
+    const int64_t kChunk = 1 << 20;
+    const int64_t nchunks = ceil_div(count, kChunk);
+    unsigned hw = std::thread::hardware_concurrency();
+    const int nthreads = (int)std::max<int64_t>(1, std::min<int64_t>(std::min<int64_t>(hw ? hw : 1, 16), nchunks));
+    std::atomic<int64_t> next{0};
+    auto work = [&]() {
+        for (int64_t c = next.fetch_add(1); c < nchunks; c = next.fetch_add(1)) body(c * kChunk, std::min(count, c * kChunk + kChunk));
+    };
+    if (nthreads <= 1) {
+        work();
+        return;
+    }
+    std::vector<std::thread> pool;
+    for (int t = 0; t < nthreads; ++t) pool.emplace_back(work);
+    for (auto& t : pool) t.join();
+}
+
 }  // namespace b2
+
+b2_index::~b2_index() {
+    if (ev0) cudaEventDestroy(ev0);
+    if (ev1) cudaEventDestroy(ev1);
+    if (stream) cudaStreamDestroy(stream);
+}
 
 // =====================================================================================================================
 extern "C" {
@@ -341,16 +416,6 @@ int b2_index_create(const void* x, int64_t n, int32_t d, int32_t dtype, int32_t 
 void b2_index_free(b2_index* idx) {
     if (!idx) return;
     DeviceGuard guard(idx->device);
-    DevBuf* bufs[] = {&idx->store, &idx->filt_pad, &idx->filt16, &idx->sub_filt16, &idx->defer, &idx->q_sub, &idx->sub_sc, &idx->sub_id, &idx->q_norm2, &idx->norm2, &idx->scalar, &idx->q_in, &idx->q_filt, &idx->cand_score,
-                      &idx->cand_id, &idx->cand_thr, &idx->flags, &idx->sel, &idx->dense, &idx->out_sc, &idx->out_id,
-                      &idx->ids_dev, &idx->sub_store, &idx->sub_filt, &idx->sub_norm2, &idx->sort_keys};
-    for (DevBuf* b : bufs) b->release();
-    idx->h_flags.release();
-    km_work_free(idx->km);
-    idx->km = nullptr;
-    if (idx->ev0) cudaEventDestroy(idx->ev0);
-    if (idx->ev1) cudaEventDestroy(idx->ev1);
-    if (idx->stream) cudaStreamDestroy(idx->stream);
     delete idx;
 }
 
@@ -473,49 +538,22 @@ int b2_index_search_stage1_dev(b2_index* idx, const void* q_dev, int64_t nq, int
     b2_index::Staged& sg = idx->staged;
     sg = b2_index::Staged();
     sg.active = true;
-    sg.q = q_dev;
-    sg.nq = nq;
-    sg.q_dtype = q_dtype;
-    sg.k = k;
     const MatView& X = idx->view;
-    const int kp = filter_kp_for_k(k);
-    const int min_splits = filter_min_splits_for_k(k);
-    const bool use_filter = kp != 0 && X.n >= 512 && ceil_div(X.n, 256) >= min_splits && X.n >= 4 * (int64_t)k;
-    const bool two_level = X.filt16 != nullptr && k <= 24 && X.n >= 4096;
-    const int64_t chunk = std::max<int64_t>(4096, std::min<int64_t>(1 << 20, (4LL << 30) / ((int64_t)std::max(min_splits, 8) * kp * 8)));
-    int dev_sms = 132;
-    cudaDeviceGetAttribute(&dev_sms, cudaDevAttrMultiProcessorCount, idx->device);
-    const bool two_cta = filter_use_pair(nq);
-    int units_whole = 0;
-    const int n_splits = use_filter ? filter_choose_splits(nq, X.n, dev_sms, two_cta, false, min_splits, &units_whole) : 0;
-    if (!use_filter || two_level || nq > chunk || n_splits <= 0 || 2 * n_splits * (kp / 2) > shard_lower_bound_max_entries() || j > k) {
+    FilterPlan& p = sg.plan;
+    B2_TRY(plan_filter(X, q_dev, q_dtype, nq, k, false, sm_count(idx->device), p));
+    if (!p.use_filter || p.two_level || p.chunks.size() != 1 || 2 * p.chunks[0].n_splits * (p.kp / 2) > shard_lower_bound_max_entries() ||
+        j > k) {
         return launch_fill_f32(lower_dev, nq, -INFINITY, st);  // stage 2 will run the plain search
     }
     idx->last_filter_ms = -1.f;
-    const int filt_dtype = X.filt_dtype;
-    const int64_t q_pitch = round_up(X.d, filt_dtype == B2_F32 ? 4 : 8);
-    const bool q_in_place = q_dtype == filt_dtype && q_pitch == X.d && (reinterpret_cast<uintptr_t>(q_dev) & 15) == 0;
-    if (!q_in_place) {
-        B2_TRY(idx->q_filt.ensure((size_t)nq * q_pitch * esize(filt_dtype)));
-        B2_TRY(launch_prep_queries(q_dev, q_dtype, nq, X.d, idx->q_filt.p, filt_dtype, q_pitch, st));
-    }
-    const void* q_filt = q_in_place ? q_dev : idx->q_filt.p;
-    B2_TRY(idx->cand_score.ensure((size_t)nq * n_splits * kp * sizeof(float)));
-    B2_TRY(idx->cand_id.ensure((size_t)nq * n_splits * kp * sizeof(int32_t)));
-    B2_TRY(idx->cand_thr.ensure((size_t)nq * n_splits * 2 * sizeof(float)));
+    const FilterChunk& c = p.chunks[0];
+    B2_TRY(run_filter(idx, p, c, idx->metric, st));
+    sg.filtered = true;
     B2_TRY(idx->q_norm2.ensure((size_t)nq * sizeof(float)));
     B2_TRY(idx->scalar.ensure(64));
-    B2_CUDA(cudaEventRecord(idx->ev0, st));
-    B2_TRY(launch_knn_filter(X, q_filt, q_pitch, nq, idx->metric, kp, n_splits, two_cta, idx->cand_score.as<float>(), idx->cand_id.as<int32_t>(),
-                             idx->cand_thr.as<float>(), idx->device, st, false, units_whole));
-    B2_CUDA(cudaEventRecord(idx->ev1, st));
-    sg.kp = kp;
-    sg.n_splits = n_splits;
-    sg.rel_eps = filter_rel_eps(X.dtype, filt_dtype, q_dtype, X.d);
-    sg.filtered = true;
     B2_TRY(launch_row_norms(q_dev, q_dtype, nq, X.d, idx->q_norm2.as<float>(), idx->scalar.as<float>() + 8, st));
-    B2_TRY(launch_shard_lower_bound(idx->cand_score.as<float>(), idx->cand_id.as<int32_t>(), nq, 2 * n_splits, kp / 2, j, idx->q_norm2.as<float>(),
-                                    X.max_norm, sg.rel_eps, idx->metric, lower_dev, st));
+    B2_TRY(launch_shard_lower_bound(idx->cand_score.as<float>(), idx->cand_id.as<int32_t>(), nq, 2 * c.n_splits, p.kp / 2, j,
+                                    idx->q_norm2.as<float>(), X.max_norm, p.rel_eps, idx->metric, lower_dev, st));
     g_stats[ST_QUERIES] += nq;
     return B2_OK;
 }
@@ -526,39 +564,18 @@ int b2_index_search_stage2_packed_dev(b2_index* idx, const float* hint_dev, uint
     idx->staged.active = false;
     if (!sg.active) { set_error("stage 2 without a stage 1"); return B2_EINVAL; }
     if (!out_packed_dev) { set_error("output buffer is NULL"); return B2_EINVAL; }
-    if (!sg.filtered) return b2_index_search_packed_dev(idx, sg.q, sg.nq, sg.q_dtype, sg.k, out_packed_dev, stream);
+    const FilterPlan& p = sg.plan;
+    if (!sg.filtered) return b2_index_search_packed_dev(idx, p.q, p.nq, p.q_dtype, p.k, out_packed_dev, stream);
     if (idx->n > 0xfffffffeLL) { set_error("packed lists hold 32-bit local ids"); return B2_ERANGE; }
     DeviceGuard guard(idx->device);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    const MatView& X = idx->view;
-    const int64_t nq = sg.nq;
-    const int k = sg.k;
-    B2_TRY(idx->out_sc.ensure((size_t)nq * k * sizeof(float)));
-    B2_TRY(idx->out_id.ensure((size_t)nq * k * sizeof(int64_t)));
-    B2_TRY(idx->flags.ensure((size_t)nq * sizeof(int32_t)));
-    B2_TRY(idx->sel.ensure((size_t)(nq + 1) * sizeof(int32_t)));
-    B2_TRY(idx->h_flags.ensure(64));
-    int32_t* sel_count = idx->sel.as<int32_t>();
-    int32_t* sel_list = sel_count + 1;
-    B2_CUDA(cudaMemsetAsync(sel_count, 0, sizeof(int32_t), st));
-    B2_TRY(launch_finalize(X, sg.q, sg.q_dtype, nq, idx->metric, k, sg.kp, sg.kp / 2, 2 * sg.n_splits, idx->cand_score.as<float>(),
-                           idx->cand_id.as<int32_t>(), idx->cand_thr.as<float>(), sg.rel_eps, nullptr, 0, idx->out_sc.as<float>(),
-                           idx->out_id.as<int64_t>(), idx->flags.as<int32_t>(), sel_list, sel_count, st, hint_dev));
-    int32_t* h_count = reinterpret_cast<int32_t*>(idx->h_flags.p);
-    B2_CUDA(cudaMemcpyAsync(h_count, sel_count, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-    cudaError_t se = cudaStreamSynchronize(st);
-    if (se != cudaSuccess) { set_error("search pipeline failed on the device: %s", cudaGetErrorString(se)); return B2_ECUDA; }
-    float ms = -1.f;
-    if (cudaEventElapsedTime(&ms, idx->ev0, idx->ev1) == cudaSuccess) idx->last_filter_ms = ms;
-    const int64_t n_sel = *h_count;
-    if (n_sel > 0) {  // uncertified queries: the exact local top-k (a superset of what the merge needs)
-        g_stats[ST_FALLBACK] += n_sel;
-        const int64_t rows = std::min<int64_t>(std::max<int64_t>(1, (int64_t)(512ull << 20) / (std::max<int64_t>(X.n, 1) * 4)), n_sel);
-        B2_TRY(idx->dense.ensure((size_t)rows * X.n * sizeof(float)));
-        B2_TRY(launch_dense_topk(X, sg.q, sg.q_dtype, nq, sel_list, n_sel, idx->metric, k, nullptr, 0, idx->dense.as<float>(), rows, nullptr,
-                                 idx->out_sc.as<float>(), idx->out_id.as<int64_t>(), st));
-    }
-    B2_TRY(launch_pack_topk(idx->out_sc.as<float>(), idx->out_id.as<int64_t>(), nq * (int64_t)k, out_packed_dev, st));
+    B2_TRY(idx->out_sc.ensure((size_t)p.nq * p.k * sizeof(float)));
+    B2_TRY(idx->out_id.ensure((size_t)p.nq * p.k * sizeof(int64_t)));
+    // uncertified queries: the exact local top-k (a superset of what the merge needs)
+    int64_t n_sel = 0;
+    B2_TRY(certify(idx, p, p.chunks[0], idx->metric, nullptr, 0, idx->out_sc.as<float>(), idx->out_id.as<int64_t>(), hint_dev,
+                   /*fallback=*/true, &n_sel, st));
+    B2_TRY(launch_pack_topk(idx->out_sc.as<float>(), idx->out_id.as<int64_t>(), p.nq * (int64_t)p.k, out_packed_dev, st));
     B2_CUDA(cudaStreamSynchronize(st));
     return B2_OK;
 }
@@ -582,9 +599,6 @@ int b2_index_gather(b2_index* idx, const int64_t* ids, int64_t m, void* out, int
     DeviceGuard guard(idx->device);
     cudaStream_t st = idx->stream;
     const size_t row_bytes = (size_t)idx->d * esize(idx->dtype);
-    B2_TRY(idx->scalar.ensure(64));
-    int* err = reinterpret_cast<int*>(idx->scalar.as<char>() + 16);
-    B2_CUDA(cudaMemsetAsync(err, 0, sizeof(int), st));
     const int64_t* ids_dev = ids;
     void* out_dev = out;
     if (!out_on_device) {
@@ -594,12 +608,11 @@ int b2_index_gather(b2_index* idx, const int64_t* ids, int64_t m, void* out, int
         B2_TRY(idx->sub_store.ensure((size_t)m * row_bytes));
         out_dev = idx->sub_store.p;
     }
-    B2_TRY(launch_gather_rows(idx->store.p, idx->dtype, idx->d, ids_dev, m, idx->n, out_dev, err, st));
-    int herr = 0;
-    B2_CUDA(cudaMemcpyAsync(&herr, err, sizeof(int), cudaMemcpyDeviceToHost, st));
-    if (!out_on_device) B2_CUDA(cudaMemcpyAsync(out, out_dev, (size_t)m * row_bytes, cudaMemcpyDeviceToHost, st));
-    B2_CUDA(cudaStreamSynchronize(st));
-    if (herr) { set_error("ids contains a position outside [0, %lld)", (long long)idx->n); return B2_ERANGE; }
+    B2_TRY(gather_rows_checked(idx->store.p, idx->dtype, idx->d, ids_dev, m, idx->n, out_dev, idx->scalar, st));
+    if (!out_on_device) {
+        B2_CUDA(cudaMemcpyAsync(out, out_dev, (size_t)m * row_bytes, cudaMemcpyDeviceToHost, st));
+        B2_CUDA(cudaStreamSynchronize(st));
+    }
     return B2_OK;
 }
 
@@ -607,35 +620,18 @@ int b2_index_gather(b2_index* idx, const int64_t* ids, int64_t m, void* out, int
 // report whether every value was already bf16-representable (then the 2-byte form is EXACT and the plugin ships it).
 int b2_host_f32_to_bf16(const float* x, int64_t count, uint16_t* out, int32_t* all_exact) {
     if (count < 0 || (count > 0 && (!x || !out))) { set_error("bad conversion arguments"); return B2_EINVAL; }
-    const int64_t kChunk = 1 << 20;
-    const int64_t nchunks = (count + kChunk - 1) / kChunk;
-    unsigned hw = std::thread::hardware_concurrency();
-    const int nthreads = (int)std::max<int64_t>(1, std::min<int64_t>(std::min<int64_t>(hw ? hw : 1, 16), nchunks));
-    std::atomic<int64_t> next{0};
     std::atomic<int> inexact{0};
-    auto work = [&]() {
-        int local_inexact = 0;
-        for (;;) {
-            const int64_t c = next.fetch_add(1);
-            if (c >= nchunks) break;
-            const int64_t lo = c * kChunk, hi = std::min(count, lo + kChunk);
-            const uint32_t* u = reinterpret_cast<const uint32_t*>(x);
-            for (int64_t i = lo; i < hi; ++i) {
-                const uint32_t v = u[i];
-                local_inexact |= (v & 0xffffu) != 0;
-                const bool is_nan = (v & 0x7fffffffu) > 0x7f800000u;
-                out[i] = is_nan ? (uint16_t)((v >> 16) | 0x0040u) : (uint16_t)((v + 0x7fffu + ((v >> 16) & 1u)) >> 16);
-            }
+    for_each_chunk(count, [&](int64_t lo, int64_t hi) {
+        const uint32_t* u = reinterpret_cast<const uint32_t*>(x);
+        int chunk_inexact = 0;
+        for (int64_t i = lo; i < hi; ++i) {
+            const uint32_t v = u[i];
+            chunk_inexact |= (v & 0xffffu) != 0;
+            const bool is_nan = (v & 0x7fffffffu) > 0x7f800000u;
+            out[i] = is_nan ? (uint16_t)((v >> 16) | 0x0040u) : (uint16_t)((v + 0x7fffu + ((v >> 16) & 1u)) >> 16);
         }
-        if (local_inexact) inexact.store(1);
-    };
-    if (nthreads <= 1) {
-        work();
-    } else {
-        std::vector<std::thread> pool;
-        for (int t = 0; t < nthreads; ++t) pool.emplace_back(work);
-        for (auto& t : pool) t.join();
-    }
+        if (chunk_inexact) inexact.store(1);
+    });
     if (all_exact) *all_exact = inexact.load() ? 0 : 1;
     return B2_OK;
 }
@@ -643,40 +639,30 @@ int b2_host_f32_to_bf16(const float* x, int64_t count, uint16_t* out, int32_t* a
 // Host-side marshalling helper: bf16 bit patterns -> float32 (exact), threaded.
 int b2_host_bf16_to_f32(const uint16_t* x, int64_t count, float* out) {
     if (count < 0 || (count > 0 && (!x || !out))) { set_error("bad conversion arguments"); return B2_EINVAL; }
-    const int64_t kChunk = 1 << 20;
-    const int64_t nchunks = (count + kChunk - 1) / kChunk;
-    unsigned hw = std::thread::hardware_concurrency();
-    const int nthreads = (int)std::max<int64_t>(1, std::min<int64_t>(std::min<int64_t>(hw ? hw : 1, 16), nchunks));
-    std::atomic<int64_t> next{0};
-    auto work = [&]() {
-        uint32_t* o = reinterpret_cast<uint32_t*>(out);
-        for (;;) {
-            const int64_t c = next.fetch_add(1);
-            if (c >= nchunks) break;
-            const int64_t lo = c * kChunk, hi = std::min(count, lo + kChunk);
-            for (int64_t i = lo; i < hi; ++i) o[i] = (uint32_t)x[i] << 16;
-        }
-    };
-    if (nthreads <= 1) {
-        work();
-    } else {
-        std::vector<std::thread> pool;
-        for (int t = 0; t < nthreads; ++t) pool.emplace_back(work);
-        for (auto& t : pool) t.join();
-    }
+    uint32_t* o = reinterpret_cast<uint32_t*>(out);
+    for_each_chunk(count, [&](int64_t lo, int64_t hi) {
+        for (int64_t i = lo; i < hi; ++i) o[i] = (uint32_t)x[i] << 16;
+    });
     return B2_OK;
 }
 
-// The filter's work schedule for a (queries, rows, k) shape on `num_sms` SMs — no device work: lets the CPU test-suite check that
-// every (query unit, corpus tile) pair is covered exactly once for the shapes the GPU tests do not reach.
+// The filter's work schedule for a (queries, rows, k) shape on `num_sms` SMs, as plan_filter decides it for a bf16 index (the
+// first query chunk when the batch takes several) — no device work: lets the CPU test-suite check that every (query unit,
+// corpus tile) pair is covered exactly once for the shapes the GPU tests do not reach.
 int b2_debug_filter_plan(int64_t nq, int64_t n, int32_t k, int32_t num_sms, int32_t* kp, int32_t* n_splits, int32_t* units_whole,
                          int32_t* two_cta) {
     if (nq <= 0 || n <= 0 || k <= 0 || num_sms <= 0 || !kp || !n_splits || !units_whole || !two_cta) { set_error("bad arguments"); return B2_EINVAL; }
-    *kp = filter_kp_for_k(k);
-    *two_cta = filter_use_pair(nq) ? 1 : 0;
-    int uw = 0;
-    *n_splits = *kp ? filter_choose_splits(nq, n, num_sms, *two_cta != 0, false, filter_min_splits_for_k(k), &uw) : 0;
-    *units_whole = uw;
+    MatView X;  // a bf16 view of n rows: one-level search
+    X.n = n;
+    X.d = 8;
+    X.dtype = X.filt_dtype = B2_BF16;
+    FilterPlan p;
+    B2_TRY(plan_filter(X, nullptr, B2_BF16, nq, k, false, num_sms, p));
+    const FilterChunk c = p.use_filter ? p.chunks[0] : FilterChunk();
+    *kp = p.use_filter ? p.kp : 0;
+    *n_splits = c.n_splits;
+    *units_whole = c.units_whole;
+    *two_cta = c.two_cta ? 1 : 0;
     return B2_OK;
 }
 

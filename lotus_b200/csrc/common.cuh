@@ -100,8 +100,6 @@ struct MatView {
                                           // the k-means loop rebuilds its centroid view every iteration)
 };
 
-struct SearchWorkspace;
-
 // ---- kernels / launchers (one per .cu) ------------------------------------------------------------------
 // knn_filter_sm90.cu
 int filter_kp_for_k(int k);  // candidate-list capacity used for a given k, 0 = k too large for the filter
@@ -112,6 +110,7 @@ bool filter_use_pair(int64_t nq);
 int filter_choose_splits(int64_t nq, int64_t n, int num_sms, bool two_cta, bool top1 = false, int min_splits = 1,
                          int* units_whole = nullptr);  // 0: impossible; *units_whole > 0: two-phase schedule (see the definition)
 int filter_min_splits_for_k(int k);
+int sm_count(int device);  // multiprocessor count of a device, cached
 int launch_pair_filter(const MatView& X, float thr, int part, int nparts, int32_t* pair_i, int32_t* pair_j,
                        unsigned long long* pair_count, unsigned long long cap, int device, cudaStream_t stream);
 

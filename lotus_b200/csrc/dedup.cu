@@ -134,31 +134,29 @@ int b2_threshold_pairs(b2_index* idx, float threshold, int32_t part, int32_t npa
     const double eps = (double)filter_rel_eps(X.dtype, X.filt_dtype, X.dtype, X.d) * (double)X.max_norm * (double)X.max_norm;
     const float thr_lo = (float)((double)threshold - eps - 1e-7 * fabs((double)threshold));
     DevBuf cand_i, cand_j, ver_i, ver_j, counters;
-    auto cleanup = [&]() { cand_i.release(); cand_j.release(); ver_i.release(); ver_j.release(); counters.release(); };
-    int rc = counters.ensure(64);
-    if (rc != B2_OK) { cleanup(); return rc; }
+    B2_TRY(counters.ensure(64));
     unsigned long long* d_cnt = counters.as<unsigned long long>();
     unsigned long long cand_cap = (unsigned long long)std::max<int64_t>(1 << 20, std::min<int64_t>(idx->n * 8, (int64_t)1 << 28));
     unsigned long long found = 0;
     for (int attempt = 0; attempt < 3; ++attempt) {
-        if ((rc = cand_i.ensure(cand_cap * sizeof(int32_t))) != B2_OK || (rc = cand_j.ensure(cand_cap * sizeof(int32_t))) != B2_OK) { cleanup(); return rc; }
-        if (cudaMemsetAsync(d_cnt, 0, 16, st) != cudaSuccess) { cleanup(); set_error("memset failed"); return B2_ECUDA; }
-        rc = launch_pair_filter(X, thr_lo, part, nparts, cand_i.as<int32_t>(), cand_j.as<int32_t>(), d_cnt, cand_cap, idx->device, st);
-        if (rc != B2_OK) { cleanup(); return rc; }
+        B2_TRY(cand_i.ensure(cand_cap * sizeof(int32_t)));
+        B2_TRY(cand_j.ensure(cand_cap * sizeof(int32_t)));
+        B2_CUDA(cudaMemsetAsync(d_cnt, 0, 16, st));
+        B2_TRY(launch_pair_filter(X, thr_lo, part, nparts, cand_i.as<int32_t>(), cand_j.as<int32_t>(), d_cnt, cand_cap, idx->device, st));
         if (cudaMemcpyAsync(&found, d_cnt, sizeof(found), cudaMemcpyDeviceToHost, st) != cudaSuccess ||
             cudaStreamSynchronize(st) != cudaSuccess) {
             set_error("pair filter failed on the device: %s", cudaGetErrorString(cudaGetLastError()));
-            cleanup();
             return B2_ECUDA;
         }
         if (found <= cand_cap) break;
         cand_cap = found + found / 8 + 1024;  // the candidate buffer overflowed: rerun with the exact size
     }
-    if (found > cand_cap) { cleanup(); set_error("pair candidate buffer overflow (%llu)", found); return B2_ENOMEM; }
+    if (found > cand_cap) { set_error("pair candidate buffer overflow (%llu)", found); return B2_ENOMEM; }
     unsigned long long kept = 0;
     std::vector<int32_t> hi, hj;
     if (found > 0) {
-        if ((rc = ver_i.ensure(found * sizeof(int32_t))) != B2_OK || (rc = ver_j.ensure(found * sizeof(int32_t))) != B2_OK) { cleanup(); return rc; }
+        B2_TRY(ver_i.ensure(found * sizeof(int32_t)));
+        B2_TRY(ver_j.ensure(found * sizeof(int32_t)));
         const int64_t blocks = std::min<int64_t>(ceil_div((int64_t)found * 32, 256), 132 * 16);
         pair_verify_kernel<<<(unsigned)blocks, 256, 0, st>>>(reinterpret_cast<const char*>(X.store), X.dtype, X.d, cand_i.as<int32_t>(),
                                                              cand_j.as<int32_t>(), (int64_t)found, threshold, ver_i.as<int32_t>(),
@@ -168,17 +166,15 @@ int b2_threshold_pairs(b2_index* idx, float threshold, int32_t part, int32_t npa
         if (cudaGetLastError() != cudaSuccess || cudaMemcpyAsync(&kept, d_cnt + 1, sizeof(kept), cudaMemcpyDeviceToHost, st) != cudaSuccess ||
             cudaStreamSynchronize(st) != cudaSuccess) {
             set_error("pair verification failed on the device: %s", cudaGetErrorString(cudaGetLastError()));
-            cleanup();
             return B2_ECUDA;
         }
         hi.resize(kept);
         hj.resize(kept);
         if (kept) {
-            cudaMemcpy(hi.data(), ver_i.p, kept * sizeof(int32_t), cudaMemcpyDeviceToHost);
-            cudaMemcpy(hj.data(), ver_j.p, kept * sizeof(int32_t), cudaMemcpyDeviceToHost);
+            B2_CUDA(cudaMemcpy(hi.data(), ver_i.p, kept * sizeof(int32_t), cudaMemcpyDeviceToHost));
+            B2_CUDA(cudaMemcpy(hj.data(), ver_j.p, kept * sizeof(int32_t), cudaMemcpyDeviceToHost));
         }
     }
-    cleanup();
     // bookkeeping on the host: order the (already exact) pair list by (i, j)
     std::vector<uint64_t> keys(kept);
     for (size_t t = 0; t < kept; ++t) keys[t] = ((uint64_t)(uint32_t)hi[t] << 32) | (uint32_t)hj[t];
@@ -201,18 +197,15 @@ int b2_connected_components(int64_t n, const int64_t* pi, const int64_t* pj, int
     if (device < 0 || device >= ndev) { set_error("device %d out of range", device); return B2_EINVAL; }
     DeviceGuard guard(device);
     DevBuf parent, dpi, dpj, dlab, derr;
-    auto cleanup = [&]() { parent.release(); dpi.release(); dpj.release(); dlab.release(); derr.release(); };
-    int rc;
-    if ((rc = parent.ensure(n * sizeof(int64_t))) != B2_OK || (rc = dlab.ensure(n * sizeof(int64_t))) != B2_OK ||
-        (rc = dpi.ensure(std::max<int64_t>(n_pairs, 1) * sizeof(int64_t))) != B2_OK ||
-        (rc = dpj.ensure(std::max<int64_t>(n_pairs, 1) * sizeof(int64_t))) != B2_OK || (rc = derr.ensure(16)) != B2_OK) {
-        cleanup();
-        return rc;
-    }
-    cudaMemset(derr.p, 0, 4);
+    B2_TRY(parent.ensure(n * sizeof(int64_t)));
+    B2_TRY(dlab.ensure(n * sizeof(int64_t)));
+    B2_TRY(dpi.ensure(std::max<int64_t>(n_pairs, 1) * sizeof(int64_t)));
+    B2_TRY(dpj.ensure(std::max<int64_t>(n_pairs, 1) * sizeof(int64_t)));
+    B2_TRY(derr.ensure(16));
+    B2_CUDA(cudaMemset(derr.p, 0, 4));
     if (n_pairs) {
-        cudaMemcpy(dpi.p, pi, n_pairs * sizeof(int64_t), cudaMemcpyHostToDevice);
-        cudaMemcpy(dpj.p, pj, n_pairs * sizeof(int64_t), cudaMemcpyHostToDevice);
+        B2_CUDA(cudaMemcpy(dpi.p, pi, n_pairs * sizeof(int64_t), cudaMemcpyHostToDevice));
+        B2_CUDA(cudaMemcpy(dpj.p, pj, n_pairs * sizeof(int64_t), cudaMemcpyHostToDevice));
     }
     const unsigned gn = (unsigned)std::min<int64_t>(ceil_div(n, 256), 132 * 16);
     uf_init_kernel<<<gn, 256>>>(parent.as<int64_t>(), n);
@@ -224,11 +217,10 @@ int b2_connected_components(int64_t n, const int64_t* pi, const int64_t* pj, int
     }
     uf_flatten_kernel<<<gn, 256>>>(parent.as<int64_t>(), dlab.as<int64_t>(), n);
     g_stats[ST_LAUNCHES]++;
-    int herr = 0;
     cudaError_t e = cudaMemcpy(labels, dlab.p, n * sizeof(int64_t), cudaMemcpyDeviceToHost);
-    cudaMemcpy(&herr, derr.p, 4, cudaMemcpyDeviceToHost);
-    cleanup();
     if (e != cudaSuccess) { set_error("connected components failed on the device: %s", cudaGetErrorString(e)); return B2_ECUDA; }
+    int herr = 0;
+    B2_CUDA(cudaMemcpy(&herr, derr.p, 4, cudaMemcpyDeviceToHost));
     if (herr) { set_error("pair list references a node outside [0, %lld)", (long long)n); return B2_ERANGE; }
     return B2_OK;
 }

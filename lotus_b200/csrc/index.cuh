@@ -1,14 +1,23 @@
 // index.cuh — the b2_index handle and the pieces of the search pipeline shared by api.cu, dedup.cu, kmeans.cu.
 #pragma once
 #include <algorithm>
+#include <memory>
+#include <vector>
 
 #include "common.cuh"
 
 namespace b2 {
 
+// Device / pinned host buffers that grow on demand and free themselves. Invariant: a buffer is destroyed while its device is
+// current. A handle's buffers go in b2_index_free under a DeviceGuard; function-local buffers are declared after the
+// DeviceGuard of their function, so they are destroyed before the guard restores the previous device.
 struct DevBuf {
     void* p = nullptr;
     size_t cap = 0;
+    DevBuf() = default;
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    ~DevBuf() { release(); }
     int ensure(size_t bytes) {
         if (bytes <= cap) return B2_OK;
         if (p) cudaFree(p);
@@ -37,6 +46,10 @@ struct DevBuf {
 struct HostBuf {
     void* p = nullptr;
     size_t cap = 0;
+    HostBuf() = default;
+    HostBuf(const HostBuf&) = delete;
+    HostBuf& operator=(const HostBuf&) = delete;
+    ~HostBuf() { release(); }
     int ensure(size_t bytes) {
         if (bytes <= cap) return B2_OK;
         if (p) cudaFreeHost(p);
@@ -58,8 +71,10 @@ struct HostBuf {
     }
 };
 
-struct KmWork;                 // kmeans.cu: per-handle k-means workspaces
-void km_work_free(KmWork* w);  // (defined in kmeans.cu)
+struct KmWork;  // kmeans.cu: per-handle k-means workspaces
+struct KmWorkDelete {
+    void operator()(KmWork* w) const;  // (defined in kmeans.cu, where KmWork is complete)
+};
 
 struct DeviceGuard {
     int prev = -1;
@@ -71,6 +86,31 @@ struct DeviceGuard {
     ~DeviceGuard() {
         if (prev >= 0) cudaSetDevice(prev);
     }
+};
+
+// One run of the top-k filter over a view, decided in one place (plan_filter) for every caller: the plain search, the staged
+// sharded search, the k-means assignment and b2_debug_filter_plan.
+struct FilterChunk {  // the queries [q0, q0 + nq) of the call, filtered by one launch
+    int64_t q0 = 0, nq = 0;
+    bool two_cta = false;
+    int n_splits = 0;
+    int units_whole = 0;  // > 0: two-phase schedule (see filter_choose_splits)
+};
+struct FilterPlan {
+    const void* q = nullptr;  // the whole query batch (device)
+    int q_dtype = B2_F32;
+    int64_t nq = 0;
+    int k = 0;
+    bool top1 = false;       // k-means assignment: register-resident top-2 epilogue, no other path
+    bool use_filter = false;  // false: the exact dense path answers every query
+    bool two_level = false;   // fp32 store with a bf16 copy: a bf16 first level with a longer list, failures go to the tf32 level
+    MatView X;                // the view the filter streams (filt = the bf16 copy on a two-level first level)
+    int kp = 0, min_splits = 1;
+    int64_t chunk = 0;  // queries per launch
+    std::vector<FilterChunk> chunks;
+    int64_t q_pitch = 0;
+    bool q_in_place = false;  // the queries already have the filter's type and a TMA-compatible pitch
+    float rel_eps = 0.f;
 };
 
 }  // namespace b2
@@ -94,16 +134,14 @@ struct b2_index {
     cudaStream_t stream = nullptr;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     float last_filter_ms = -1.f;
-    b2::KmWork* km = nullptr;
+    std::unique_ptr<b2::KmWork, b2::KmWorkDelete> km;
     // row-sharded search in two stages (b2_index_search_stage1_dev / _stage2_packed_dev): what stage 1 left for stage 2
     struct Staged {
-        bool active = false, filtered = false;  // filtered: the candidate lists of (q, nq, k) are in the workspace
-        const void* q = nullptr;
-        int64_t nq = 0;
-        int32_t q_dtype = 0, k = 0, kp = 0, n_splits = 0;
-        float rel_eps = 0.f;
+        bool active = false, filtered = false;  // filtered: the candidate lists of plan's (q, nq, k) are in the workspace
+        b2::FilterPlan plan;
     } staged;
     DevBuf q_norm2;
+    ~b2_index();  // destroys the stream and events; the buffers free themselves
 };
 
 namespace b2 {
@@ -117,5 +155,11 @@ int build_view(const void* store, int64_t n, int d, int dtype, DevBuf& filt_pad,
 int search_core(b2_index* idx, const MatView& X, int metric, const void* q_dev, int q_dtype, int64_t nq, int k,
                 const int64_t* id_map, int64_t id_offset, float* out_sc, int64_t* out_id, cudaStream_t st, int level = 0);
 float filter_rel_eps(int store_dtype, int filt_dtype, int q_dtype, int d);
+int plan_filter(const MatView& X, const void* q, int q_dtype, int64_t nq, int k, bool top1, int num_sms, FilterPlan& plan);
+// prep one chunk's queries (unless streamed in place), size the candidate workspace and run the filter between idx->ev0 and ev1
+int run_filter(b2_index* idx, const FilterPlan& plan, const FilterChunk& c, int metric, cudaStream_t st);
+// out[j] = x[ids[j]] for j < m, synchronised; ids outside [0, n) -> B2_ERANGE. scalar holds the device error flag.
+int gather_rows_checked(const void* x, int dtype, int d, const int64_t* ids, int64_t m, int64_t n, void* out, DevBuf& scalar,
+                        cudaStream_t st);
 
 }  // namespace b2

@@ -32,22 +32,11 @@ namespace b2 {
 
 struct KmWork {
     DevBuf cent[2], cent_filt, cent_norm2, scalar, pts, pts_norm2, train, train_norm2, assign, members, offsets, totals, blk, hassign, ids,
-        obj, flag_ids, flag_count, hard_ids, order, dbg, sub, sub_dis, sub_assign, fin_assign, fin_dis, perm;
+        obj, flag_ids, flag_count, hard_ids, order, sub, sub_dis, sub_assign, fin_assign, fin_dis, perm;
     HostBuf h_count;
-    void release() {
-        DevBuf* all[] = {&cent[0], &cent[1], &cent_filt, &cent_norm2, &scalar, &pts, &pts_norm2, &train, &train_norm2, &assign, &members,
-                         &offsets, &totals, &blk, &hassign, &ids, &obj, &flag_ids, &flag_count, &hard_ids, &order, &dbg, &sub, &sub_dis, &sub_assign, &fin_assign,
-                         &fin_dis, &perm};
-        for (DevBuf* b : all) b->release();
-        h_count.release();
-    }
 };
 
-void km_work_free(KmWork* w) {
-    if (!w) return;
-    w->release();
-    delete w;
-}
+void KmWorkDelete::operator()(KmWork* w) const { delete w; }
 
 namespace {
 
@@ -300,7 +289,7 @@ __global__ void km_fill_kernel(const int64_t* assign, int64_t n, int64_t L, int 
 //     have already landed;
 //   * balance: cluster sizes are far from equal while Lloyd is converging (some centroids hold 4x the mean), and the longest
 //     chain bounds the pass — warps pull items off a device counter in DECREASING cluster size (km_order_kernel).
-// History (profiles/r2_kmeans_accumulate_variants.txt, all at 5M x 768 bf16, k = 1024, one pass):
+// History (measured on a B200, all at 5M x 768 bf16, k = 1024, one pass):
 //   r1  thread per (centroid, column), 2-byte loads ................................ 9.4 ms
 //   v1  block per centroid, 16 row loads per lane in registers ..................... 5.3 ms  (DRAM 18 %, SMs busy 29 % of the time)
 //   v2  same shape, cp.async ring of 32 rows per block ............................. 6.6 ms  (the per-centroid chain, not load depth, bounds it)
@@ -308,7 +297,7 @@ __global__ void km_fill_kernel(const int64_t* assign, int64_t n, int64_t L, int 
 //   v5  + per-column objective partials (one fp32 chain over a group's 64 products was the critical path), 32-bit ids,
 //       unpredicated full groups, 6 warps x 64-row rings per SM .................... 3.6 ms   <- this kernel
 //   also tried: 4- and 8-byte lanes (4x / 2x as many, thinner chains), 256-row rings, branch-free predicated copies, TMA bulk
-//   copies (cp.async.bulk + mbarrier, one copy per row slice): 3.6-5.0 ms, none better. Per-item counters (B2_KM_DEBUG=1) show
+//   copies (cp.async.bulk + mbarrier, one copy per row slice): 3.6-5.0 ms, none better. Per-item cycle counters showed
 //   why: the largest cluster holds ~48k of the 5M rows (10x the mean) and its chain advances at 110-170 cycles per row whatever
 //   the variant, so the pass cannot end before ~48k x 140 cycles = 3.5 ms; the other 3071 items finish long before.
 // With OBJ the same pass accumulates sum_members ||x - c_old||^2 (fp32 partials per group, summed in fp64: fp64 issue is scarce).
@@ -360,7 +349,7 @@ template <bool BF16, bool OBJ, int LB, int ACC_GROUPS>
 __global__ void __launch_bounds__(256) km_accumulate_vec_kernel(const void* x, int d, const int64_t* ids, const int32_t* members,
                                                                 const int64_t* offsets, const int32_t* order, const float* cent_old,
                                                                 float* cent_out, float* hassign, double* obj, int normalize, int k,
-                                                                int n_chunks, int* work_counter, long long* dbg) {
+                                                                int n_chunks, int* work_counter) {
     constexpr int V = BF16 ? LB / 2 : LB / 4;  // columns per lane
     using Word = typename LaneWord<LB>::T;
     extern __shared__ __align__(16) uint8_t acc_ring_raw[];  // [warps][ACC_GROUPS * ACC_ROWS][32] words
@@ -374,7 +363,6 @@ __global__ void __launch_bounds__(256) km_accumulate_vec_kernel(const void* x, i
         if (lane == 0) item = atomicAdd(work_counter, 1);
         item = __shfl_sync(FULL, item, 0);
         if (item >= n_items) break;
-        const long long dbg_t0 = dbg ? clock64() : 0;
         const int c = order[item / n_chunks];
         const int chunk = item - (item / n_chunks) * n_chunks;
         const int word = chunk * 32 + lane;  // this lane's LB-byte slice inside a row
@@ -487,14 +475,6 @@ __global__ void __launch_bounds__(256) km_accumulate_vec_kernel(const void* x, i
 #pragma unroll
             for (int off = 16; off >= 1; off >>= 1) dsum += __shfl_xor_sync(FULL, dsum, off);
             if (lane == 0 && dsum != 0.0) atomicAdd(obj, dsum);
-        }
-        if (dbg && lane == 0) {  // B2_KM_DEBUG: (rows, cycles, start clock, SM) of every work item
-            unsigned smid;
-            asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
-            dbg[4 * (size_t)item + 0] = nmem;
-            dbg[4 * (size_t)item + 1] = clock64() - dbg_t0;
-            dbg[4 * (size_t)item + 2] = dbg_t0;
-            dbg[4 * (size_t)item + 3] = smid;
         }
         __syncwarp();
     }
@@ -675,15 +655,10 @@ int assign_points(b2_index* idx, const void* pts, const float* pnorm2, int64_t m
     const int d = idx->d;
     MatView cv;
     B2_TRY(centroid_view(cent, k, d, idx->dtype, w, cv, st));
-    int dev_sms = 132;
-    cudaDeviceGetAttribute(&dev_sms, cudaDevAttrMultiProcessorCount, idx->device);
-    const int filt_dtype = cv.filt_dtype;
-    const int kp = 16;
-    const int64_t q_pitch = round_up(d, filt_dtype == B2_F32 ? 4 : 8);
-    const float rel_eps = filter_rel_eps(B2_F32, filt_dtype, idx->dtype, d);
-    const bool q_in_place = idx->dtype == filt_dtype && q_pitch == d && (reinterpret_cast<uintptr_t>(pts) & 15) == 0;
-    const int64_t chunk = (int64_t)1 << 23;
-    B2_TRY(w.flag_ids.ensure((size_t)std::min(m, chunk) * sizeof(int32_t)));
+    const int dev_sms = sm_count(idx->device);
+    FilterPlan p;
+    B2_TRY(plan_filter(cv, pts, idx->dtype, m, 1, /*top1=*/true, dev_sms, p));
+    B2_TRY(w.flag_ids.ensure((size_t)std::min(m, p.chunk) * sizeof(int32_t)));
     B2_TRY(w.hard_ids.ensure((size_t)m * sizeof(int64_t)));
     B2_TRY(w.flag_count.ensure(64));
     B2_TRY(w.h_count.ensure(64));
@@ -697,36 +672,22 @@ int assign_points(b2_index* idx, const void* pts, const float* pnorm2, int64_t m
         return B2_ERANGE;
     }
     if (rk_smem > 48 * 1024) B2_CUDA(cudaFuncSetAttribute(km_rescore_known_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rk_smem));
-    B2_CUDA(cudaEventRecord(idx->ev0, st));
-    for (int64_t q0 = 0; q0 < m; q0 += chunk) {
-        const int64_t mc = std::min<int64_t>(chunk, m - q0);
-        const char* pc = reinterpret_cast<const char*>(pts) + (size_t)q0 * d * esize(idx->dtype);
-        const bool two_cta = filter_use_pair(mc);
-        const int n_splits = filter_choose_splits(mc, k, dev_sms, two_cta, /*top1=*/true);
-        if (!q_in_place) {
-            B2_TRY(idx->q_filt.ensure((size_t)mc * q_pitch * esize(filt_dtype)));
-            B2_TRY(launch_prep_queries(pc, idx->dtype, mc, d, idx->q_filt.p, filt_dtype, q_pitch, st));
-        }
-        const void* q_filt = q_in_place ? static_cast<const void*>(pc) : idx->q_filt.p;
-        B2_TRY(idx->cand_score.ensure((size_t)mc * n_splits * kp * sizeof(float)));
-        B2_TRY(idx->cand_id.ensure((size_t)mc * n_splits * kp * sizeof(int32_t)));
-        B2_TRY(idx->cand_thr.ensure((size_t)mc * n_splits * 2 * sizeof(float)));
-        B2_TRY(launch_knn_filter(cv, q_filt, q_pitch, mc, B2_METRIC_L2, kp, n_splits, two_cta, idx->cand_score.as<float>(),
-                                 idx->cand_id.as<int32_t>(), idx->cand_thr.as<float>(), idx->device, st, /*top1=*/true));
-        if (q0 + chunk >= m) B2_CUDA(cudaEventRecord(idx->ev1, st));
-        if (q0 > 0) B2_CUDA(cudaMemsetAsync(flag_count, 0, sizeof(int32_t), st));
-        km_assign_finalize_kernel<<<(unsigned)ceil_div(mc, 256), 256, 0, st>>>(
-            idx->cand_score.as<float>(), idx->cand_id.as<int32_t>(), idx->cand_thr.as<float>(), mc, 2 * n_splits, kp / 2, pnorm2,
-            cv.max_norm_dev, rel_eps, assign, w.flag_ids.as<int32_t>(), flag_count, q0);
+    for (const FilterChunk& c : p.chunks) {
+        B2_TRY(run_filter(idx, p, c, B2_METRIC_L2, st));
+        if (c.q0 > 0) B2_CUDA(cudaMemsetAsync(flag_count, 0, sizeof(int32_t), st));
+        const int n_lists = 2 * c.n_splits, list_len = p.kp / 2;
+        km_assign_finalize_kernel<<<(unsigned)ceil_div(c.nq, 256), 256, 0, st>>>(
+            idx->cand_score.as<float>(), idx->cand_id.as<int32_t>(), idx->cand_thr.as<float>(), c.nq, n_lists, list_len, pnorm2,
+            cv.max_norm_dev, p.rel_eps, assign, w.flag_ids.as<int32_t>(), flag_count, c.q0);
         B2_LAUNCH_CHECK();
         // the flagged points of this chunk, while its candidate lists are still in the workspace (count read on the device)
-        if (4 * n_splits <= 32)
+        if (2 * n_lists <= 32)
             km_rescore_known_kernel<<<dev_sms * 4, 256, rk_smem, st>>>(pts, idx->dtype, d, cent, idx->cand_score.as<float>(),
-                                                                     idx->cand_id.as<int32_t>(), idx->cand_thr.as<float>(), 2 * n_splits, kp / 2,
-                                                                     pnorm2, cv.max_norm_dev, rel_eps, w.flag_ids.as<int32_t>(), flag_count, q0,
+                                                                     idx->cand_id.as<int32_t>(), idx->cand_thr.as<float>(), n_lists, list_len,
+                                                                     pnorm2, cv.max_norm_dev, p.rel_eps, w.flag_ids.as<int32_t>(), flag_count, c.q0,
                                                                      assign, w.hard_ids.as<int64_t>(), hard_count);
         else
-            km_forward_flags_kernel<<<dev_sms, 256, 0, st>>>(w.flag_ids.as<int32_t>(), flag_count, q0, w.hard_ids.as<int64_t>(), hard_count);
+            km_forward_flags_kernel<<<dev_sms, 256, 0, st>>>(w.flag_ids.as<int32_t>(), flag_count, c.q0, w.hard_ids.as<int64_t>(), hard_count);
         B2_LAUNCH_CHECK();
     }
     int32_t* h_count = reinterpret_cast<int32_t*>(w.h_count.p);
@@ -791,14 +752,9 @@ int update_centroids(b2_index* idx, const void* x, const int64_t* row_ids, int64
     B2_LAUNCH_CHECK();
     // Bytes of a member row per lane: 16 (a warp covers 512 B of the row, fewest instructions per byte) unless that leaves too few
     // (centroid, chunk) chains to occupy the machine — few centroids — then 4 (128 B per warp, 4x as many chains).
-    // B2_KM_LANE_BYTES = 4 | 16 overrides. Measured at 5M x 768, k = 1024 (profiles/r2_kmeans_accumulate_variants.txt): the pass is
-    // bounded by the LARGEST cluster's chain (~48k of 5M rows, 10x the mean, while Lloyd converges) at ~110-170 cycles per row of
-    // one warp, whatever the lane width (4 / 8 / 16 B), the ring depth (64 / 256 rows) or the copy mechanism (cp.async / TMA bulk).
-    static const int lane_bytes_env = [] { const char* e = getenv("B2_KM_LANE_BYTES"); const int v = e ? atoi(e) : 0; return (v == 4 || v == 16) ? v : 0; }();
     const size_t row_bytes_total = (size_t)d * esize(idx->dtype);
-    int sms = 132;
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, idx->device);
-    int LB = lane_bytes_env ? lane_bytes_env : ((int64_t)k * (int64_t)ceil_div((int64_t)row_bytes_total, 512) >= 4LL * 6 * sms ? 16 : 4);
+    const int sms = sm_count(idx->device);
+    int LB = (int64_t)k * (int64_t)ceil_div((int64_t)row_bytes_total, 512) >= 4LL * 6 * sms ? 16 : 4;
     if (LB == 16 && (row_bytes_total % 16 != 0 || (reinterpret_cast<uintptr_t>(x) % 16) != 0)) LB = 4;
     const bool vec_ok = row_bytes_total % LB == 0 && (reinterpret_cast<uintptr_t>(x) % LB) == 0;
     if (vec_ok) {
@@ -814,12 +770,6 @@ int update_centroids(b2_index* idx, const void* x, const int64_t* row_ids, int64
         B2_CUDA(cudaMemsetAsync(counter, 0, sizeof(int), st));
         km_order_kernel<<<1, 1024, 0, st>>>(w.totals.as<int32_t>(), k, w.order.as<int32_t>());
         B2_LAUNCH_CHECK();
-        static const bool dbg_on = [] { const char* e = getenv("B2_KM_DEBUG"); return e && atoi(e) != 0; }();
-        long long* dbg = nullptr;
-        if (dbg_on) {
-            B2_TRY(w.dbg.ensure((size_t)k * n_chunks * 4 * sizeof(long long)));
-            dbg = w.dbg.as<long long>();
-        }
 #define B2_ACC_LAUNCH(BF, OB, LBV, NGV)                                                                                           \
     do {                                                                                                                          \
         auto kern = km_accumulate_vec_kernel<BF, OB, LBV, NGV>;                                                                   \
@@ -829,7 +779,7 @@ int update_centroids(b2_index* idx, const void* x, const int64_t* row_ids, int64
         per_sm = std::max(1, std::min<int>(per_sm, (int)(ACC_SMEM / ring)));                                                      \
         const int grid = (int)std::min<int64_t>(ceil_div((int64_t)k * n_chunks, warps), (int64_t)per_sm * sms);                   \
         kern<<<grid, warps * 32, ring, st>>>(x, d, row_ids, w.members.as<int32_t>(), w.offsets.as<int64_t>(), w.order.as<int32_t>(), \
-                                             cent_old, cent_out, w.hassign.as<float>(), obj, normalize, k, n_chunks, counter, dbg); \
+                                             cent_old, cent_out, w.hassign.as<float>(), obj, normalize, k, n_chunks, counter);      \
     } while (0)
 #define B2_ACC_LB(BF, OB)                              \
     do {                                               \
@@ -845,20 +795,6 @@ int update_centroids(b2_index* idx, const void* x, const int64_t* row_ids, int64
         }
 #undef B2_ACC_LB
 #undef B2_ACC_LAUNCH
-        if (dbg) {
-            std::vector<long long> h((size_t)k * n_chunks * 4);
-            cudaStreamSynchronize(st);
-            cudaMemcpy(h.data(), dbg, h.size() * sizeof(long long), cudaMemcpyDeviceToHost);
-            long long rows_tot = 0;
-            size_t worst = 0;
-            for (size_t i = 0; i < (size_t)k * n_chunks; ++i) {
-                rows_tot += h[4 * i];
-                if (h[4 * i + 1] > h[4 * worst + 1]) worst = i;
-            }
-            fprintf(stderr, "[b2 km accumulate dbg] lane bytes %d, items %d, rows/item mean %.0f | slowest item: %lld rows in %lld cycles (%.0f cycles/row), SM %lld\n",
-                    LB, k * n_chunks, (double)rows_tot / (k * n_chunks), h[4 * worst], h[4 * worst + 1],
-                    (double)h[4 * worst + 1] / std::max<long long>(h[4 * worst], 1), h[4 * worst + 3]);
-        }
     } else {
         dim3 grid((unsigned)k, (unsigned)ceil_div(d, 128));
         km_accumulate_kernel<<<grid, 128, 0, st>>>(x, idx->dtype, d, row_ids, w.members.as<int32_t>(), w.offsets.as<int64_t>(), cent_old,
@@ -905,18 +841,8 @@ int point_set(b2_index* idx, const int64_t* ids_dev, int64_t m, KmWork& w, const
     const int d = idx->d;
     B2_TRY(w.pts.ensure((size_t)std::max<int64_t>(m, 1) * d * esize(idx->dtype)));
     B2_TRY(w.pts_norm2.ensure((size_t)std::max<int64_t>(m, 1) * sizeof(float)));
-    B2_TRY(w.scalar.ensure(64));
-    int* err = reinterpret_cast<int*>(w.scalar.as<char>() + 16);
-    B2_CUDA(cudaMemsetAsync(err, 0, sizeof(int), st));
-    B2_TRY(launch_gather_rows(idx->store.p, idx->dtype, d, ids_dev, m, idx->n, w.pts.p, err, st));
+    B2_TRY(gather_rows_checked(idx->store.p, idx->dtype, d, ids_dev, m, idx->n, w.pts.p, w.scalar, st));
     B2_TRY(launch_row_norms(w.pts.p, idx->dtype, m, d, w.pts_norm2.as<float>(), w.scalar.as<float>() + 8, st));
-    int herr = 0;
-    B2_CUDA(cudaMemcpyAsync(&herr, err, sizeof(int), cudaMemcpyDeviceToHost, st));
-    B2_CUDA(cudaStreamSynchronize(st));
-    if (herr) {
-        set_error("ids contains a position outside [0, %lld)", (long long)idx->n);
-        return B2_ERANGE;
-    }
     P = w.pts.p;
     Pn = w.pts_norm2.as<float>();
     return B2_OK;
@@ -1010,7 +936,7 @@ int kmeans_impl(b2_index* idx, const int64_t* ids_host, int64_t m, int k, int ni
 }
 
 KmWork& work_of(b2_index* idx) {
-    if (!idx->km) idx->km = new KmWork();
+    if (!idx->km) idx->km.reset(new KmWork());
     return *idx->km;
 }
 
@@ -1021,6 +947,32 @@ int check_ids_host(b2_index* idx, const int64_t* ids, int64_t m) {
             set_error("ids contains a position outside [0, %lld)", (long long)idx->n);
             return B2_ERANGE;
         }
+    return B2_OK;
+}
+
+// b2_kmeans_assign on host arrays: copies in, b2_kmeans_assign_dev, copies out (the caller holds the DeviceGuard)
+int kmeans_assign_host(b2_index* idx, const int64_t* ids, int64_t m, const float* centroids, int k, int64_t* out_assign,
+                       float* out_dist, KmWork& w) {
+    cudaStream_t st = idx->stream;
+    const int d = idx->d;
+    DevBuf cent, dis, asg;
+    B2_TRY(cent.ensure((size_t)k * d * sizeof(float)));
+    if (out_dist) B2_TRY(dis.ensure((size_t)m * sizeof(float)));
+    B2_TRY(asg.ensure((size_t)m * sizeof(int64_t)));
+    const int64_t* ids_dev = nullptr;
+    if (ids) {
+        B2_TRY(w.ids.ensure((size_t)m * sizeof(int64_t)));
+        B2_CUDA(cudaMemcpyAsync(w.ids.p, ids, (size_t)m * sizeof(int64_t), cudaMemcpyHostToDevice, st));
+        ids_dev = w.ids.as<int64_t>();
+    }
+    B2_CUDA(cudaMemcpyAsync(cent.p, centroids, (size_t)k * d * sizeof(float), cudaMemcpyHostToDevice, st));
+    B2_TRY(b2_kmeans_assign_dev(idx, ids_dev, m, cent.as<float>(), k, asg.as<int64_t>(), out_dist ? dis.as<float>() : nullptr, st));
+    B2_CUDA(cudaMemcpyAsync(out_assign, asg.p, (size_t)m * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    if (out_dist) B2_CUDA(cudaMemcpyAsync(out_dist, dis.p, (size_t)m * sizeof(float), cudaMemcpyDeviceToHost, st));
+    if (cudaStreamSynchronize(st) != cudaSuccess) {
+        set_error("k-means assignment failed on the device: %s", cudaGetErrorString(cudaGetLastError()));
+        return B2_ECUDA;
+    }
     return B2_OK;
 }
 
@@ -1095,35 +1047,24 @@ int b2_kmeans_accumulate(b2_index* idx, const int64_t* ids, int64_t m, const int
     cudaStream_t st = idx->stream;
     KmWork& w = work_of(idx);
     DevBuf d_assign, d_sums, d_counts;
-    int rc = d_assign.ensure((size_t)std::max<int64_t>(m, 1) * sizeof(int64_t));
-    if (rc == B2_OK) rc = d_sums.ensure((size_t)k * idx->d * sizeof(float));
-    if (rc == B2_OK) rc = d_counts.ensure((size_t)k * sizeof(float));
+    B2_TRY(d_assign.ensure((size_t)std::max<int64_t>(m, 1) * sizeof(int64_t)));
+    B2_TRY(d_sums.ensure((size_t)k * idx->d * sizeof(float)));
+    B2_TRY(d_counts.ensure((size_t)k * sizeof(float)));
     const int64_t* ids_dev = nullptr;
-    if (rc == B2_OK && ids) {
-        rc = w.ids.ensure((size_t)std::max<int64_t>(m, 1) * sizeof(int64_t));
-        if (rc == B2_OK) {
-            cudaMemcpyAsync(w.ids.p, ids, (size_t)m * sizeof(int64_t), cudaMemcpyHostToDevice, st);
-            ids_dev = w.ids.as<int64_t>();
-        }
+    if (ids) {
+        B2_TRY(w.ids.ensure((size_t)std::max<int64_t>(m, 1) * sizeof(int64_t)));
+        B2_CUDA(cudaMemcpyAsync(w.ids.p, ids, (size_t)m * sizeof(int64_t), cudaMemcpyHostToDevice, st));
+        ids_dev = w.ids.as<int64_t>();
     }
-    if (rc == B2_OK) {
-        cudaMemcpyAsync(d_assign.p, assign, (size_t)m * sizeof(int64_t), cudaMemcpyHostToDevice, st);
-        rc = b2_kmeans_accumulate_dev(idx, ids_dev, m, d_assign.as<int64_t>(), k, nullptr, d_sums.as<float>(), d_counts.as<float>(), nullptr, st);
+    B2_CUDA(cudaMemcpyAsync(d_assign.p, assign, (size_t)m * sizeof(int64_t), cudaMemcpyHostToDevice, st));
+    B2_TRY(b2_kmeans_accumulate_dev(idx, ids_dev, m, d_assign.as<int64_t>(), k, nullptr, d_sums.as<float>(), d_counts.as<float>(), nullptr, st));
+    B2_CUDA(cudaMemcpyAsync(out_sums, d_sums.p, (size_t)k * idx->d * sizeof(float), cudaMemcpyDeviceToHost, st));
+    B2_CUDA(cudaMemcpyAsync(out_counts, d_counts.p, (size_t)k * sizeof(float), cudaMemcpyDeviceToHost, st));
+    if (cudaStreamSynchronize(st) != cudaSuccess) {
+        set_error("k-means accumulate failed on the device: %s", cudaGetErrorString(cudaGetLastError()));
+        return B2_ECUDA;
     }
-    if (rc == B2_OK) {
-        cudaMemcpyAsync(out_sums, d_sums.p, (size_t)k * idx->d * sizeof(float), cudaMemcpyDeviceToHost, st);
-        cudaMemcpyAsync(out_counts, d_counts.p, (size_t)k * sizeof(float), cudaMemcpyDeviceToHost, st);
-        if (cudaStreamSynchronize(st) != cudaSuccess) {
-            set_error("k-means accumulate failed on the device: %s", cudaGetErrorString(cudaGetLastError()));
-            rc = B2_ECUDA;
-        }
-    } else {
-        cudaStreamSynchronize(st);
-    }
-    d_assign.release();
-    d_sums.release();
-    d_counts.release();
-    return rc;
+    return B2_OK;
 }
 
 int b2_kmeans_assign(b2_index* idx, const int64_t* ids, int64_t m, const float* centroids, int32_t k, int64_t* out_assign,
@@ -1134,35 +1075,12 @@ int b2_kmeans_assign(b2_index* idx, const int64_t* ids, int64_t m, const float* 
     if (m == 0) return B2_OK;
     B2_TRY(check_ids_host(idx, ids, m));
     DeviceGuard guard(idx->device);
-    cudaStream_t st = idx->stream;
-    const int d = idx->d;
     KmWork& w = work_of(idx);
-    DevBuf cent, dis, asg;
-    auto cleanup = [&]() { cudaStreamSynchronize(st); cent.release(); dis.release(); asg.release(); w.pts.release(); w.pts_norm2.release(); };
-    int rc = cent.ensure((size_t)k * d * sizeof(float));
-    if (rc == B2_OK && out_dist) rc = dis.ensure((size_t)m * sizeof(float));
-    if (rc == B2_OK) rc = asg.ensure((size_t)m * sizeof(int64_t));
-    const int64_t* ids_dev = nullptr;
-    if (rc == B2_OK && ids) {
-        rc = w.ids.ensure((size_t)m * sizeof(int64_t));
-        if (rc == B2_OK) {
-            cudaMemcpyAsync(w.ids.p, ids, (size_t)m * sizeof(int64_t), cudaMemcpyHostToDevice, st);
-            ids_dev = w.ids.as<int64_t>();
-        }
-    }
-    if (rc == B2_OK) {
-        cudaMemcpyAsync(cent.p, centroids, (size_t)k * d * sizeof(float), cudaMemcpyHostToDevice, st);
-        rc = b2_kmeans_assign_dev(idx, ids_dev, m, cent.as<float>(), k, asg.as<int64_t>(), out_dist ? dis.as<float>() : nullptr, st);
-    }
-    if (rc == B2_OK) {
-        cudaMemcpyAsync(out_assign, asg.p, (size_t)m * sizeof(int64_t), cudaMemcpyDeviceToHost, st);
-        if (out_dist) cudaMemcpyAsync(out_dist, dis.p, (size_t)m * sizeof(float), cudaMemcpyDeviceToHost, st);
-        if (cudaStreamSynchronize(st) != cudaSuccess) {
-            set_error("k-means assignment failed on the device: %s", cudaGetErrorString(cudaGetLastError()));
-            rc = B2_ECUDA;
-        }
-    }
-    cleanup();
+    const int rc = kmeans_assign_host(idx, ids, m, centroids, k, out_assign, out_dist, w);
+    cudaStreamSynchronize(idx->stream);
+    // the gathered point set is per call
+    w.pts.release();
+    w.pts_norm2.release();
     return rc;
 }
 

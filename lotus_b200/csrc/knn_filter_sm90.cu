@@ -798,6 +798,8 @@ int launch_two(int kp, bool is_l2, bool tf32, const CUtensorMap& tq, const CUten
     }
 }
 
+}  // namespace
+
 int sm_count(int device) {
     static int cached[64] = {0};
     if (device >= 0 && device < 64 && cached[device]) return cached[device];
@@ -806,8 +808,6 @@ int sm_count(int device) {
     if (device >= 0 && device < 64) cached[device] = n;
     return n;
 }
-
-}  // namespace
 
 int filter_kp_for_k(int k) {
     if (k <= 6) return 16;
@@ -837,19 +837,6 @@ bool filter_use_pair(int64_t nq) {
 // In pair mode a worker is a CTA pair and a query unit is two query tiles.
 int filter_choose_splits(int64_t nq, int64_t n, int num_sms, bool two_cta, bool top1, int min_splits, int* units_whole) {
     if (units_whole) *units_whole = 0;
-    {
-        static int forced = -1;  // B2_FILTER_SPLITS: experiments only
-        if (forced < 0) {
-            const char* e = getenv("B2_FILTER_SPLITS");
-            forced = e ? atoi(e) : 0;
-        }
-        if (forced > 0) {
-            const int64_t nt = ceil_div(n, BLOCK_N);
-            int s = (int)std::min<int64_t>(forced, nt);
-            while (s > 1 && ceil_div(nt, ceil_div(nt, s)) != s) --s;
-            return s;
-        }
-    }
     const int64_t n_mtiles = ceil_div(nq, BLOCK_M);
     const int64_t n_units = two_cta ? ceil_div(n_mtiles, 2) : n_mtiles;
     const int64_t workers = two_cta ? std::max(1, num_sms / 2) : num_sms;
@@ -874,9 +861,8 @@ int filter_choose_splits(int64_t nq, int64_t n, int num_sms, bool two_cta, bool 
     // wave instead of one per split, and the workers still stream the same corpus tiles in step, which is what keeps them in
     // L2); only the leftover units (< one per worker) are cut into splits, just fine enough to fill the last waves. On a
     // 125k-row shard with 100k queries: 5 x (489 + 13) + 2 x (70 + 13) = 2676 tile-times against 16 x (163 + 13) = 2816.
-    static const bool two_phase_on = [] { const char* e = getenv("B2_FILTER_TWO_PHASE"); return e ? atoi(e) != 0 : true; }();
     const int64_t waves_a = n_units / workers;
-    if (units_whole && two_phase_on && min_splits <= 1 && waves_a >= 1) {
+    if (units_whole && min_splits <= 1 && waves_a >= 1) {
         const int64_t ua = waves_a * workers, rem = n_units - ua;
         const double cost_a = (double)waves_a * ((double)n_ntiles + kWarmupTiles);
         double best2 = 1e300;
