@@ -24,8 +24,9 @@
 //
 // Epilogue lists: the wgmma fragment spreads a query row over four lanes, so each warp passes its 16 rows x 256 scores
 // through a small shared-memory transpose, 16 columns at a time; afterwards lane (r, e) = (lane & 15, lane >> 4) holds 8
-// scores of row r. Candidate list ("set") e of a row collects the columns c with bit 3 of c equal to e, so a query keeps
-// two lists of KP/2 per corpus split, the layout finalize merges.
+// scores of row r. Before a chunk is transposed, each lane tests its fragment values against the thresholds of their
+// lists, and one warp vote skips the chunk when none can enter. Candidate list ("set") e of a row collects the columns c
+// with bit 3 of c equal to e, so a query keeps two lists of KP/2 per corpus split, the layout finalize merges.
 #include <cuda.h>
 
 #include "common.cuh"
@@ -82,10 +83,16 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 // arrive on the barrier at the same offset in CTA `cta` of the cluster
+//
+// Plain arrive (default .release.cta semantics), not .release.cluster: ptxas lowers the cluster-scope release to a
+// GPU-wide MEMBAR that the consumers would then pay at every stage release, in the middle of the wgmma pipeline. Nothing
+// here needs that ordering. The only accesses to order are this CTA's wgmma reads of the stage against the peer's later
+// TMA multicast into it: wgmma.wait_group has retired those reads before the arrive is made, and the peer's producer
+// waits on this barrier before it issues the copy. No data written through memory has to become visible to anyone.
 __device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
     uint32_t remote;
     asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(bar)), "r"(cta));
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
+    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
 }
 // Bounded wait: a protocol bug must trap (sticky error the host reports) instead of hanging the GPU. No printf here: a
 // function call inside the consumers' wgmma pipeline makes ptxas serialize every wgmma.
@@ -470,16 +477,12 @@ __device__ __forceinline__ void prepare8(float (&v)[8], int idx0, int valid, con
     }
 }
 
-// Eight consecutive scores of the lane's (row, set). One warp vote skips the group when no lane beats its threshold (late
-// in a sweep almost always); otherwise 8 branch-free predicated appends into the pending buffer and one vote on a flush.
+// Eight consecutive scores of the lane's (row, set), in a chunk where some lane of the warp beats its threshold (the
+// consumer's gate skips the others): 8 branch-free predicated appends into the pending buffer and one vote on a flush.
 // The pending buffers are merged into the lists by the whole warp in lockstep once any lane holds PEND_FLUSH candidates.
 template <int KPH>
 __device__ __forceinline__ void process8(const float (&v)[8], int idx0, float* my_sc, int32_t* my_id, float* pend_sc,
                                          int32_t* pend_id, float& thr, int& minpos, int& cnt) {
-    float m = v[0];
-#pragma unroll
-    for (int j = 1; j < 8; ++j) m = fmaxf(m, v[j]);
-    if (!__any_sync(0xffffffffu, m > thr)) return;
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
         if (v[j] > thr) {  // cnt <= PEND_FLUSH - 1 on entry: the pending buffer cannot overflow
@@ -572,12 +575,34 @@ knn_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
             int cnt = 0;      // pending candidates of this (row, set)
             float b1 = -INFINITY, b2 = -INFINITY, b3 = -INFINITY;  // TOP1: best two scores + discard bound
             int32_t i1 = -1, i2 = -1;
+            // thresholds of the lists this lane's fragment values go to: gthr[h][s] is (row fr + 8h, set s), the `thr` of
+            // lane fr + 8h + 16s
+            float gthr[2][2] = {{-INFINITY, -INFINITY}, {-INFINITY, -INFINITY}};
             for (int t = t0; t < t1; ++t) {
                 mma_tile<TF32, NSTAGES, TWO>(acc, ring, p.num_kb, g, sc.rank, stage, phase);
                 const int col0 = t * BLOCK_N;
                 const int ncols = min(BLOCK_N, p.n - col0);
 #pragma unroll
                 for (int c = 0; c < BLOCK_N / 16; ++c) {  // 16-column chunks through the per-warp transpose
+                    if constexpr (!TOP1) {
+                        // Gate: test the chunk's fragment values, as prepare8 transforms them, against the thresholds of
+                        // their lists. When no lane holds a value above its threshold (late in a sweep almost always),
+                        // process8 would append nothing, so the chunk skips the transpose and is done.
+                        bool hit = false;
+#pragma unroll
+                        for (int jj = 0; jj < 2; ++jj) {
+#pragma unroll
+                            for (int h = 0; h < 4; ++h) {  // acc[a + h]: row fr + 8 (h >> 1), column 16c + 8jj + fc + (h & 1)
+                                const int off = 16 * c + 8 * jj + fc + (h & 1);
+                                float s = acc[(2 * c + jj) * 4 + h];
+                                if constexpr (IS_L2) {
+                                    if (off < ncols) s = fmaf(2.f, s, -__ldg(p.xnorm + col0 + off));
+                                }
+                                hit |= off < ncols && s > gthr[h >> 1][jj];
+                            }
+                        }
+                        if (!__any_sync(0xffffffffu, hit)) continue;
+                    }
                     __syncwarp();
 #pragma unroll
                     for (int jj = 0; jj < 2; ++jj) {
@@ -593,10 +618,17 @@ knn_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
                     for (int j = 0; j < 8; ++j) v[j] = xs[rr * XP_STRIDE + 8 * e + j];
                     const int off = 16 * c + 8 * e;
                     prepare8<IS_L2>(v, col0 + off, ncols - off, p.xnorm);
-                    if constexpr (TOP1)
+                    if constexpr (TOP1) {
                         process8_top2(v, col0 + off, b1, b2, b3, i1, i2);
-                    else
+                    } else {
                         process8<KPH>(v, col0 + off, my_sc, my_id, pend_sc, pend_id, thr, minpos, cnt);
+                        // a flush may have raised the thresholds the gate tests against
+#pragma unroll
+                        for (int h = 0; h < 2; ++h) {
+#pragma unroll
+                            for (int s = 0; s < 2; ++s) gthr[h][s] = __shfl_sync(0xffffffffu, thr, fr + 8 * h + 16 * s);
+                        }
+                    }
                 }
             }
             if constexpr (TOP1) {
