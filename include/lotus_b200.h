@@ -195,6 +195,15 @@ B2_API int b2_host_bf16_to_f32(const uint16_t* x, int64_t count, float* out);
  * item each (two-phase schedule), two_cta = CTA-pair mode. */
 B2_API int b2_debug_filter_plan(int64_t nq, int64_t n, int32_t k, int32_t num_sms, int32_t* kp, int32_t* n_splits,
                          int32_t* units_whole, int32_t* two_cta);
+/* The filter kernel's raw candidate lists for host queries q[nq,d] (q_dtype), planned and launched exactly as a search does
+ * (level 0; level 1 = the tf32 second level of an fp32 index, which drops its bf16 copy) or, with top1 != 0, as the k-means
+ * assignment does (register top-2 epilogue). plan[8] receives: use_filter, kp, n_splits, units_whole, two_cta, two_level,
+ * filter operand dtype, query chunks; *rel_eps the filter's error bound relative to |q|*|x|. With every list buffer non-NULL
+ * and use_filter set, the filter runs and fills (HOST buffers) cand_score / cand_id [nq, n_splits, 2 sets, kp/2] and
+ * cand_thr [nq, n_splits, 2]; with any of them NULL only the plan is reported. B2_ERANGE when nq needs more than one query
+ * chunk. For testing; not part of the search path. */
+B2_API int b2_debug_filter_lists(b2_index* idx, const void* q, int64_t nq, int32_t q_dtype, int32_t k, int32_t top1, int32_t level,
+                          int32_t* plan, float* rel_eps, float* cand_score, int32_t* cand_id, float* cand_thr);
 
 /* ---- instrumentation ---------------------------------------------------------------------------------- */
 /* counters since the last b2_stats_reset(): [0] kernels launched by this library, [1] queries answered,

@@ -21,6 +21,7 @@ SYMBOLS = [
     "b2_index_ntotal", "b2_index_dim", "b2_index_dtype", "b2_index_metric", "b2_index_device", "b2_index_data_dev",
     "b2_index_search", "b2_index_search_dev", "b2_merge_topk_dev", "b2_index_search_packed_dev", "b2_merge_topk_packed_dev", "b2_index_search_stage1_dev", "b2_index_search_stage2_packed_dev", "b2_index_gather", "b2_threshold_pairs",
     "b2_connected_components", "b2_kmeans", "b2_kmeans_assign", "b2_kmeans_accumulate", "b2_kmeans_assign_dev", "b2_kmeans_accumulate_dev", "b2_stats", "b2_stats_reset", "b2_last_filter_ms", "b2_host_f32_to_bf16", "b2_host_bf16_to_f32", "b2_debug_filter_plan",
+    "b2_debug_filter_lists",
 ]
 
 
@@ -94,6 +95,8 @@ def lib() -> ctypes.CDLL:
     L.b2_host_bf16_to_f32.argtypes = [vp, i64, vp]
     L.b2_debug_filter_plan.restype = c.c_int
     L.b2_debug_filter_plan.argtypes = [i64, i64, i32, i32, c.POINTER(i32), c.POINTER(i32), c.POINTER(i32), c.POINTER(i32)]
+    L.b2_debug_filter_lists.restype = c.c_int
+    L.b2_debug_filter_lists.argtypes = [vp, vp, i64, i32, i32, i32, i32, c.POINTER(i32), c.POINTER(f32), vp, vp, vp]
     L.b2_stats.restype = c.c_int
     L.b2_stats.argtypes = [c.POINTER(i64), i32]
     L.b2_stats_reset.restype = None
@@ -244,6 +247,32 @@ class Index:
         ids = np.ascontiguousarray(ids, dtype=np.int64)
         out = np.empty((len(ids), self.d), dtype=np.float32 if self.dtype == F32 else np.uint16)
         check(lib().b2_index_gather(self._h, _ptr(ids), len(ids), _ptr(out), 0))
+        return out
+
+    def filter_lists(self, q: np.ndarray, k: int, q_dtype: int = F32, top1: bool = False, level: int = 0,
+                     plan_only: bool = False) -> dict:
+        """The filter kernel's raw candidate lists for host queries, run as a search (or, with top1, the k-means assignment)
+        runs it: the plan (use_filter, kp, n_splits, units_whole, two_cta, two_level, filt_dtype, rel_eps) plus, unless
+        plan_only or the plan declines the filter, score/id [nq, n_splits, 2, kp/2] and thr [nq, n_splits, 2]."""
+        q = np.ascontiguousarray(q)
+        nq = q.shape[0]
+        if q.ndim != 2 or q.shape[1] != self.d:
+            raise ValueError(f"queries must be [nq, {self.d}]")
+        plan = (ctypes.c_int32 * 8)()
+        eps = ctypes.c_float()
+        L = lib()
+        check(L.b2_debug_filter_lists(self._h, _ptr(q), nq, q_dtype, k, int(top1), level, plan, ctypes.byref(eps), None, None, None))
+        out = {"use_filter": bool(plan[0]), "kp": plan[1], "n_splits": plan[2], "units_whole": plan[3], "two_cta": bool(plan[4]),
+               "two_level": bool(plan[5]), "filt_dtype": plan[6], "rel_eps": float(eps.value)}
+        if plan_only or not out["use_filter"]:
+            return out
+        ns, kph = out["n_splits"], out["kp"] // 2
+        sc = np.empty((nq, ns, 2, kph), dtype=np.float32)
+        ids = np.empty((nq, ns, 2, kph), dtype=np.int32)
+        thr = np.empty((nq, ns, 2), dtype=np.float32)
+        check(L.b2_debug_filter_lists(self._h, _ptr(q), nq, q_dtype, k, int(top1), level, plan, ctypes.byref(eps), _ptr(sc),
+                                      _ptr(ids), _ptr(thr)))
+        out.update(score=sc, id=ids, thr=thr)
         return out
 
     def last_filter_ms(self) -> float:

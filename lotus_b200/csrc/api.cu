@@ -72,8 +72,9 @@ int build_view(const void* store, int64_t n, int d, int dtype, DevBuf& filt_pad,
 // relative (to ||q||*||x||) bound on |filter score - exact score| of the inner product
 float filter_rel_eps(int store_dtype, int filt_dtype, int q_dtype, int d) {
     // fp32 accumulation inside the tensor core: products are exact, every accumulation step may lose one
-    // (truncated) ulp of the running magnitude; (d + 64) * 2^-23 is generous. Exercised by tests/test_gpu_search.py and
-    // tests/test_gpu_fuzz.py: a too-small bound shows up as a wrong neighbour, a too-large one only as fallback work.
+    // (truncated) ulp of the running magnitude; (d + 64) * 2^-23 is generous. tests/test_gpu_filter_lists.py checks every
+    // list entry against this bound in its per-row form (|x| of the row, not max |x|) and pins the formula; the largest
+    // measured |err| is 0.66 rel_eps |q| |x| (DESIGN.md §2).
     const double acc = (double)(d + 64) * 1.1920929e-7;
     double ex = 0.0, eq = 0.0;  // relative representation error of the corpus / query operand seen by the MMA
     if (filt_dtype == B2_F32) {  // tf32 wgmma keeps 10 explicit mantissa bits of an fp32 operand
@@ -663,6 +664,46 @@ int b2_debug_filter_plan(int64_t nq, int64_t n, int32_t k, int32_t num_sms, int3
     *n_splits = c.n_splits;
     *units_whole = c.units_whole;
     *two_cta = c.two_cta ? 1 : 0;
+    return B2_OK;
+}
+
+// The raw candidate lists of one filter run on host queries, planned and launched exactly as search_core (level 0 / 1) or the
+// k-means assignment (top1) does it, so the tests can check the kernel's contract list by list instead of through finalize.
+int b2_debug_filter_lists(b2_index* idx, const void* q, int64_t nq, int32_t q_dtype, int32_t k, int32_t top1, int32_t level,
+                          int32_t* plan, float* rel_eps, float* cand_score, int32_t* cand_id, float* cand_thr) {
+    B2_TRY(check_search_args(idx, q, nq, q_dtype, k));
+    if (nq == 0 || !plan || !rel_eps || (level != 0 && level != 1)) { set_error("bad arguments"); return B2_EINVAL; }
+    const bool lists = cand_score && cand_id && cand_thr;
+    DeviceGuard guard(idx->device);
+    cudaStream_t st = idx->stream;
+    MatView X = idx->view;
+    if (level == 1 || top1) X.filt16 = nullptr;  // the second level drops the bf16 copy; the k-means centroid view has none
+    const size_t qbytes = (size_t)nq * idx->d * esize(q_dtype);
+    if (lists) {
+        B2_TRY(idx->q_in.ensure(qbytes));
+        B2_CUDA(cudaMemcpyAsync(idx->q_in.p, q, qbytes, cudaMemcpyHostToDevice, st));
+    }
+    FilterPlan p;
+    B2_TRY(plan_filter(X, lists ? idx->q_in.p : nullptr, q_dtype, nq, k, top1 != 0, sm_count(idx->device), p));
+    const FilterChunk c = p.use_filter ? p.chunks[0] : FilterChunk();
+    plan[0] = p.use_filter ? 1 : 0;
+    plan[1] = p.use_filter ? p.kp : 0;
+    plan[2] = c.n_splits;
+    plan[3] = c.units_whole;
+    plan[4] = c.two_cta ? 1 : 0;
+    plan[5] = p.two_level ? 1 : 0;
+    plan[6] = p.X.filt_dtype;
+    plan[7] = (int32_t)p.chunks.size();
+    *rel_eps = p.rel_eps;
+    if (p.chunks.size() > 1) { set_error("%lld queries take %zu query chunks; one is supported", (long long)nq, p.chunks.size()); return B2_ERANGE; }
+    if (!lists || !p.use_filter) return B2_OK;
+    B2_TRY(run_filter(idx, p, c, idx->metric, st));
+    const size_t entries = (size_t)nq * c.n_splits * p.kp;
+    B2_CUDA(cudaMemcpyAsync(cand_score, idx->cand_score.p, entries * sizeof(float), cudaMemcpyDeviceToHost, st));
+    B2_CUDA(cudaMemcpyAsync(cand_id, idx->cand_id.p, entries * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    B2_CUDA(cudaMemcpyAsync(cand_thr, idx->cand_thr.p, (size_t)nq * c.n_splits * 2 * sizeof(float), cudaMemcpyDeviceToHost, st));
+    cudaError_t e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) { set_error("filter failed on the device: %s", cudaGetErrorString(e)); return B2_ECUDA; }
     return B2_OK;
 }
 

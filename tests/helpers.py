@@ -20,6 +20,26 @@ def bits(a):
     return np.ascontiguousarray(a, dtype=np.float32).view(np.uint32)
 
 
+def schedule_items(plan, nq, n, workers):
+    """Python mirror of knn_filter_sm90.cu item_range / num_items (non-pair mode): -> per worker the list of (unit, split, t0, t1)."""
+    n_mtiles = -(-nq // 128)
+    n_units = -(-n_mtiles // 2) if plan["two_cta"] else n_mtiles
+    n_ntiles = -(-n // 256)
+    s, uw = plan["n_splits"], plan["units_whole"]
+    tps = -(-n_ntiles // s)
+    total = uw + (n_units - uw) * s
+    out = [[] for _ in range(workers)]
+    for item in range(total):
+        if item < uw:
+            unit, split, t0, t1 = item, 0, 0, n_ntiles
+        else:
+            j, rem = item - uw, n_units - uw
+            unit, split = uw + j % rem, j // rem
+            t0, t1 = split * tps, min(split * tps + tps, n_ntiles)
+        out[item % workers].append((unit, split, t0, t1))
+    return out, n_units, n_ntiles
+
+
 class NumpyVS:
     """Test double of the VS plugin surface (lotus/vector_store/vs.py) backed by the oracle: lets the pandas
     operators be exercised on CPU. It lives in tests/ only — the product has no CPU path."""

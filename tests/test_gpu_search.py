@@ -64,7 +64,8 @@ def test_filter_path_gaussian(gpu, dtype, metric, k):
 
 @pytest.mark.parametrize("dtype,d", [("bf16", 768), ("f32", 768), ("bf16", 100), ("f32", 30), ("bf16", 384)])
 def test_filter_path_dims(gpu, dtype, d):
-    check(gpu, gauss(9001, d, 4), gauss(257, d, 5), 10, 0, dtype, expect_filter=True)
+    st = check(gpu, gauss(9001, d, 4), gauss(257, d, 5), 10, 0, dtype, expect_filter=True)
+    assert st["fallback_queries"] <= 3, st  # measured 0 of 257 for every (dtype, d) (H100 80GB HBM3, 400 W)
 
 
 @pytest.mark.parametrize("metric", [0, 1])
@@ -87,8 +88,9 @@ def test_unnormalised_and_duplicate_rows(gpu):
     x[3999] = x[0]
     q = np.concatenate([x[[7, 0]], gauss(30, 64, 9, normalize=False)])
     for metric in (0, 1):
-        check(gpu, x, q, 5, metric, "f32")
-        check(gpu, x, q, 5, metric, "bf16")
+        for dtype in ("f32", "bf16"):
+            st = check(gpu, x, q, 5, metric, dtype, expect_filter=True)
+            assert st["fallback_queries"] <= 2, st  # measured 0 of 32 in all four runs (H100 80GB HBM3, 400 W)
 
 
 def test_ids_subset_semantics(gpu):

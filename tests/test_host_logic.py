@@ -10,7 +10,7 @@ import pytest
 
 import lotus_b200 as lotus
 import oracle
-from helpers import NumpyVS, gauss
+from helpers import NumpyVS, gauss, schedule_items
 from lotus_b200 import faiss_io
 
 
@@ -449,26 +449,6 @@ def test_sem_search_k_doubling_branch_equals_the_ids_branch_and_rerank_reorders(
         lotus.settings.configure(reranker=None)
 
 
-def _schedule_items(plan, nq, n, workers):
-    """Python mirror of knn_filter_sm90.cu item_range / num_items (non-pair mode): -> per worker the list of (unit, split, t0, t1)."""
-    n_mtiles = -(-nq // 128)
-    n_units = -(-n_mtiles // 2) if plan["two_cta"] else n_mtiles
-    n_ntiles = -(-n // 256)
-    s, uw = plan["n_splits"], plan["units_whole"]
-    tps = -(-n_ntiles // s)
-    total = uw + (n_units - uw) * s
-    out = [[] for _ in range(workers)]
-    for item in range(total):
-        if item < uw:
-            unit, split, t0, t1 = item, 0, 0, n_ntiles
-        else:
-            j, rem = item - uw, n_units - uw
-            unit, split = uw + j % rem, j // rem
-            t0, t1 = split * tps, min(split * tps + tps, n_ntiles)
-        out[item % workers].append((unit, split, t0, t1))
-    return out, n_units, n_ntiles
-
-
 @pytest.mark.parametrize("nq,n", [(100_000, 1_000_000), (100_000, 500_000), (100_000, 250_000), (100_000, 125_000), (40_000, 20_000),
                                   (18_944, 3_000), (19_200, 70_000), (9_472, 500_000), (300, 6_000), (1_000_000, 4_096)])
 @pytest.mark.parametrize("k", [10, 32, 64])
@@ -480,7 +460,7 @@ def test_filter_schedule_covers_every_unit_tile_pair_once(nq, n, k):
     plan = nv.filter_plan(nq, n, k)
     assert plan["kp"] > 0 and plan["n_splits"] >= 1
     workers = 66 if plan["two_cta"] else 132
-    per_worker, n_units, n_ntiles = _schedule_items(plan, nq, n, workers)
+    per_worker, n_units, n_ntiles = schedule_items(plan, nq, n, workers)
     assert plan["units_whole"] % workers == 0 and 0 <= plan["units_whole"] <= n_units
     cover = np.zeros((n_units, n_ntiles), dtype=np.int32)
     lists = set()
