@@ -55,8 +55,12 @@ extern "C" {
 #define B2_API
 #endif
 
-/* element types of embedding matrices */
-enum { B2_F32 = 0, B2_BF16 = 1 };
+/* element types of embedding matrices. B2_F16 is IEEE binary16: its values and their pairwise products are exact in fp32,
+ * so an fp16 index is searched on the 2-byte tensor-core path with no operand error, and the results are those of the
+ * fp32 upcast of the stored values. fp32 / bf16 queries on an fp16 index are rounded to fp16 for the filter only (a query
+ * component of magnitude >= 65520 sends that query to the exact dense path); the reported scores always use the
+ * query as given. */
+enum { B2_F32 = 0, B2_BF16 = 1, B2_F16 = 2 };
 /* metrics; numeric values match faiss.METRIC_INNER_PRODUCT / faiss.METRIC_L2 */
 enum { B2_METRIC_IP = 0, B2_METRIC_L2 = 1 };
 
@@ -204,6 +208,11 @@ B2_API int b2_debug_filter_plan(int64_t nq, int64_t n, int32_t k, int32_t num_sm
  * chunk. For testing; not part of the search path. */
 B2_API int b2_debug_filter_lists(b2_index* idx, const void* q, int64_t nq, int32_t q_dtype, int32_t k, int32_t top1, int32_t level,
                           int32_t* plan, float* rel_eps, float* cand_score, int32_t* cand_id, float* cand_thr);
+/* The filter's error model for one operand combination (no device work): |filter score - exact inner product| <=
+ * rel_eps * |q| * |x| + abs_eps * (|q| + |x|) for a store of `store_dtype` filtered as `filt_dtype` (B2_F32 = tf32 wgmma,
+ * B2_BF16 / B2_F16 = 2-byte wgmma) with queries of `q_dtype`, dimension d. abs_eps is non-zero only where an operand is
+ * rounded to fp16 (its subnormal spacing). For testing; the search paths use the same function. */
+B2_API int b2_debug_filter_eps(int32_t store_dtype, int32_t filt_dtype, int32_t q_dtype, int32_t d, float* rel_eps, float* abs_eps);
 
 /* ---- instrumentation ---------------------------------------------------------------------------------- */
 /* counters since the last b2_stats_reset(): [0] kernels launched by this library, [1] queries answered,

@@ -11,7 +11,8 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libb2lotus.so")
 
-F32, BF16 = 0, 1
+F32, BF16, F16 = 0, 1, 2
+DTYPES = (F32, BF16, F16)
 METRIC_IP, METRIC_L2 = 0, 1
 OK, EINVAL, ENODEV, ECUDA, ENOMEM, ERANGE = 0, -1, -2, -3, -4, -5
 
@@ -21,7 +22,7 @@ SYMBOLS = [
     "b2_index_ntotal", "b2_index_dim", "b2_index_dtype", "b2_index_metric", "b2_index_device", "b2_index_data_dev",
     "b2_index_search", "b2_index_search_dev", "b2_merge_topk_dev", "b2_index_search_packed_dev", "b2_merge_topk_packed_dev", "b2_index_search_stage1_dev", "b2_index_search_stage2_packed_dev", "b2_index_gather", "b2_threshold_pairs",
     "b2_connected_components", "b2_kmeans", "b2_kmeans_assign", "b2_kmeans_accumulate", "b2_kmeans_assign_dev", "b2_kmeans_accumulate_dev", "b2_stats", "b2_stats_reset", "b2_last_filter_ms", "b2_host_f32_to_bf16", "b2_host_bf16_to_f32", "b2_debug_filter_plan",
-    "b2_debug_filter_lists",
+    "b2_debug_filter_lists", "b2_debug_filter_eps",
 ]
 
 
@@ -97,6 +98,8 @@ def lib() -> ctypes.CDLL:
     L.b2_debug_filter_plan.argtypes = [i64, i64, i32, i32, c.POINTER(i32), c.POINTER(i32), c.POINTER(i32), c.POINTER(i32)]
     L.b2_debug_filter_lists.restype = c.c_int
     L.b2_debug_filter_lists.argtypes = [vp, vp, i64, i32, i32, i32, i32, c.POINTER(i32), c.POINTER(f32), vp, vp, vp]
+    L.b2_debug_filter_eps.restype = c.c_int
+    L.b2_debug_filter_eps.argtypes = [i32, i32, i32, i32, c.POINTER(f32), c.POINTER(f32)]
     L.b2_stats.restype = c.c_int
     L.b2_stats.argtypes = [c.POINTER(i64), i32]
     L.b2_stats_reset.restype = None
@@ -125,6 +128,13 @@ def filter_plan(nq: int, n: int, k: int, num_sms: int = 132) -> dict:
     kp, ns, uw, two = ctypes.c_int32(), ctypes.c_int32(), ctypes.c_int32(), ctypes.c_int32()
     check(lib().b2_debug_filter_plan(nq, n, k, num_sms, ctypes.byref(kp), ctypes.byref(ns), ctypes.byref(uw), ctypes.byref(two)))
     return {"kp": kp.value, "n_splits": ns.value, "units_whole": uw.value, "two_cta": bool(two.value)}
+
+
+def filter_eps(store_dtype: int, filt_dtype: int, q_dtype: int, d: int) -> tuple[float, float]:
+    """(rel_eps, abs_eps) of the filter's error model for an operand combination (host logic only, no device needed)."""
+    rel, ab = ctypes.c_float(), ctypes.c_float()
+    check(lib().b2_debug_filter_eps(store_dtype, filt_dtype, q_dtype, d, ctypes.byref(rel), ctypes.byref(ab)))
+    return float(rel.value), float(ab.value)
 
 
 def stats() -> dict:
@@ -166,6 +176,31 @@ def bf16_bits_to_f32(b: np.ndarray) -> np.ndarray:
     return out
 
 
+def storage_dtype(code: int) -> np.dtype:
+    """numpy dtype of a matrix's elements as the C-ABI holds them: float32, bfloat16 bit patterns (uint16; numpy has no
+    bfloat16) or float16."""
+    if code == F32:
+        return np.dtype(np.float32)
+    if code == BF16:
+        return np.dtype(np.uint16)
+    if code == F16:
+        return np.dtype(np.float16)
+    raise ValueError(f"unknown element type code {code}")
+
+
+def stored_to_f32(a: np.ndarray, code: int) -> np.ndarray:
+    """float32 values of a matrix stored as element type `code` (exact for every type): the one place that knows how each
+    type's storage turns into numbers."""
+    if code == F32:
+        return np.ascontiguousarray(a, dtype=np.float32)
+    if code == BF16:
+        return bf16_bits_to_f32(a)
+    if code == F16:
+        a = np.ascontiguousarray(a)
+        return (a.view(np.float16) if a.dtype == np.uint16 else a.astype(np.float16, copy=False)).astype(np.float32)
+    raise ValueError(f"unknown element type code {code}")
+
+
 def _ptr(a: Optional[np.ndarray]):
     return None if a is None else ctypes.c_void_p(a.ctypes.data)
 
@@ -182,7 +217,9 @@ class Index:
             check(L.b2_index_create(ctypes.c_void_p(on_device_ptr), n, d, dtype, metric, device, 1, ctypes.byref(self._h)))
         else:
             x = np.ascontiguousarray(x)
-            want = np.float32 if dtype == F32 else np.uint16
+            want = storage_dtype(dtype)
+            if dtype == F16 and x.dtype == np.uint16:  # fp16 bit patterns are accepted as well
+                x = x.view(np.float16)
             if x.dtype != want:
                 raise TypeError(f"matrix must be {want} for dtype {dtype}, got {x.dtype}")
             if x.ndim != 2:
@@ -245,7 +282,7 @@ class Index:
 
     def gather(self, ids) -> np.ndarray:
         ids = np.ascontiguousarray(ids, dtype=np.int64)
-        out = np.empty((len(ids), self.d), dtype=np.float32 if self.dtype == F32 else np.uint16)
+        out = np.empty((len(ids), self.d), dtype=storage_dtype(self.dtype))
         check(lib().b2_index_gather(self._h, _ptr(ids), len(ids), _ptr(out), 0))
         return out
 

@@ -39,7 +39,7 @@ int build_view(const void* store, int64_t n, int d, int dtype, DevBuf& filt_pad,
     v.d = d;
     v.dtype = dtype;
     v.filt_dtype = dtype;
-    const int align = dtype == B2_F32 ? 4 : 8;  // TMA row pitch must be a multiple of 16 bytes
+    const int align = tma_align_elems(dtype);  // TMA row pitch must be a multiple of 16 bytes
     if (d % align == 0) {
         v.filt = store;
         v.filt_pitch = d;
@@ -69,6 +69,19 @@ int build_view(const void* store, int64_t n, int d, int dtype, DevBuf& filt_pad,
     return B2_OK;
 }
 
+// Relative representation error of one operand of `dtype` seen by a wgmma of `filt_dtype`: 0 when the value is exact.
+//   tf32 keeps 10 explicit mantissa bits of an fp32 value (2^-10); bf16 and fp16 values are exact in tf32.
+//   bf16 wgmma: fp32 values are rounded to bf16 (2^-8); fp16 values (11-bit significand) are rounded too, also 2^-8.
+//   fp16 wgmma: fp32 and bf16 values are rounded to fp16 (2^-11 relative, plus the absolute term of filter_abs_eps for the
+//   subnormal range). bf16 values that are fp16-normal would be exact, but a bf16 value can lie outside fp16's range.
+static double operand_rel_err(int dtype, int filt_dtype) {
+    switch (filt_dtype) {
+        case B2_F32: return dtype == B2_F32 ? 9.765625e-4 : 0.0;
+        case B2_BF16: return dtype == B2_BF16 ? 0.0 : 3.90625e-3;
+        default: return dtype == B2_F16 ? 0.0 : 4.8828125e-4;  // B2_F16
+    }
+}
+
 // relative (to ||q||*||x||) bound on |filter score - exact score| of the inner product
 float filter_rel_eps(int store_dtype, int filt_dtype, int q_dtype, int d) {
     // fp32 accumulation inside the tensor core: products are exact, every accumulation step may lose one
@@ -76,15 +89,20 @@ float filter_rel_eps(int store_dtype, int filt_dtype, int q_dtype, int d) {
     // list entry against this bound in its per-row form (|x| of the row, not max |x|) and pins the formula; the largest
     // measured |err| is 0.66 rel_eps |q| |x| (DESIGN.md §2).
     const double acc = (double)(d + 64) * 1.1920929e-7;
-    double ex = 0.0, eq = 0.0;  // relative representation error of the corpus / query operand seen by the MMA
-    if (filt_dtype == B2_F32) {  // tf32 wgmma keeps 10 explicit mantissa bits of an fp32 operand
-        ex = store_dtype == B2_F32 ? 9.765625e-4 : 0.0;  // bf16 values are exact in tf32
-        eq = q_dtype == B2_F32 ? 9.765625e-4 : 0.0;
-    } else {  // bf16 wgmma on bf16 operands
-        ex = store_dtype == B2_F32 ? 3.90625e-3 : 0.0;  // fp32 values rounded to bf16 for the filter
-        eq = q_dtype == B2_F32 ? 3.90625e-3 : 0.0;
-    }
+    // relative representation error of the corpus / query operand seen by the MMA
+    const double ex = operand_rel_err(store_dtype, filt_dtype), eq = operand_rel_err(q_dtype, filt_dtype);
     return (float)(acc + ex + eq + ex * eq + 1e-6);
+}
+
+// Absolute part of the bound, in |filter - exact| <= rel_eps |q| |x| + abs_eps (|q| + |x|). Rounding v to fp16 (round to
+// nearest even) errs by at most 2^-11 |v| + 2^-25 (half the subnormal spacing 2^-24), so a rounded side adds at most
+// 2^-25 * sum_i |other_i| <= 2^-25 sqrt(d) |other| to the inner product. Zero unless a side is rounded to fp16. (No search
+// rounds both sides: an fp16 filter streams an fp16 store or, in k-means, fp32 centroids against fp16 points; the cross term
+// of two rounded sides would need more than this.)
+float filter_abs_eps(int store_dtype, int filt_dtype, int q_dtype, int d) {
+    if (filt_dtype != B2_F16) return 0.f;
+    const int rounded = (store_dtype != B2_F16 ? 1 : 0) + (q_dtype != B2_F16 ? 1 : 0);
+    return (float)(rounded * 2.9802322387695312e-8 * sqrt((double)d) * (1.0 + 1e-6));
 }
 
 // deferred[j] = base + sel[j] (chunk-local query numbers -> batch-wide)
@@ -135,9 +153,11 @@ int plan_filter(const MatView& X_in, const void* q, int q_dtype, int64_t nq, int
     // with k well below the rows of a split. The k-means assignment has no other path.
     p.use_filter = top1 || (p.kp != 0 && X.n >= 512 && ceil_div(X.n, 256) >= p.min_splits && X.n >= 4 * (int64_t)k);
     if (!p.use_filter) return B2_OK;
-    p.q_pitch = round_up(X.d, X.filt_dtype == B2_F32 ? 4 : 8);
+    p.q_pitch = round_up(X.d, tma_align_elems(X.filt_dtype));
     p.q_in_place = q_dtype == X.filt_dtype && p.q_pitch == X.d && (reinterpret_cast<uintptr_t>(q) & 15) == 0;
     p.rel_eps = filter_rel_eps(X.dtype, X.filt_dtype, q_dtype, X.d);
+    p.abs_eps = filter_abs_eps(X.dtype, X.filt_dtype, q_dtype, X.d);
+    if (X.filt_dtype == B2_F16 && q_dtype != B2_F16) p.q_norm_limit = 65504.f;  // rounded queries: see FilterPlan
     // bound the candidate workspace (nqc x n_splits x kp x 8 bytes) to a few GB: fewer queries per chunk when k needs many splits
     p.chunk = top1 ? (int64_t)1 << 23
                    : std::max<int64_t>(4096, std::min<int64_t>(1 << 20, (4LL << 30) / ((int64_t)std::max(p.min_splits, 8) * p.kp * 8)));
@@ -197,7 +217,7 @@ static int certify(b2_index* idx, const FilterPlan& p, const FilterChunk& c, int
     int32_t* sel_list = sel_count + 1;
     B2_CUDA(cudaMemsetAsync(sel_count, 0, sizeof(int32_t), st));
     B2_TRY(launch_finalize(X, qc, p.q_dtype, c.nq, metric, p.k, p.kp, p.kp / 2, 2 * c.n_splits, idx->cand_score.as<float>(),
-                           idx->cand_id.as<int32_t>(), idx->cand_thr.as<float>(), p.rel_eps, id_map, id_offset, osc, oid,
+                           idx->cand_id.as<int32_t>(), idx->cand_thr.as<float>(), p.rel_eps, p.abs_eps, p.q_norm_limit, id_map, id_offset, osc, oid,
                            idx->flags.as<int32_t>(), sel_list, sel_count, st, hint));
     // the certificate outcome comes back as ONE counter (the failed queries are compacted on the device)
     int32_t* h_count = reinterpret_cast<int32_t*>(idx->h_flags.p);
@@ -368,7 +388,7 @@ int b2_index_create(const void* x, int64_t n, int32_t d, int32_t dtype, int32_t 
     if (!out) { set_error("out is NULL"); return B2_EINVAL; }
     *out = nullptr;
     if (n < 0 || d <= 0 || (n > 0 && !x)) { set_error("bad matrix shape n=%lld d=%d", (long long)n, d); return B2_EINVAL; }
-    if (dtype != B2_F32 && dtype != B2_BF16) { set_error("dtype must be B2_F32 or B2_BF16"); return B2_EINVAL; }
+    if (!dtype_valid(dtype)) { set_error("dtype must be B2_F32, B2_BF16 or B2_F16"); return B2_EINVAL; }
     if (metric != B2_METRIC_IP && metric != B2_METRIC_L2) { set_error("metric must be B2_METRIC_IP or B2_METRIC_L2"); return B2_EINVAL; }
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
@@ -431,7 +451,7 @@ float b2_last_filter_ms(const b2_index* idx) { return idx ? idx->last_filter_ms 
 static int check_search_args(b2_index* idx, const void* q, int64_t nq, int32_t q_dtype, int32_t k) {
     if (!idx) { set_error("Index not loaded"); return B2_EINVAL; }
     if (nq < 0 || (nq > 0 && !q)) { set_error("bad query batch"); return B2_EINVAL; }
-    if (q_dtype != B2_F32 && q_dtype != B2_BF16) { set_error("q_dtype must be B2_F32 or B2_BF16"); return B2_EINVAL; }
+    if (!dtype_valid(q_dtype)) { set_error("q_dtype must be B2_F32, B2_BF16 or B2_F16"); return B2_EINVAL; }
     if (k <= 0) { set_error("k must be positive (got %d)", k); return B2_EINVAL; }
     if (k > dense_max_k()) { set_error("k=%d is not supported (max %d)", k, dense_max_k()); return B2_ERANGE; }
     return B2_OK;
@@ -554,7 +574,7 @@ int b2_index_search_stage1_dev(b2_index* idx, const void* q_dev, int64_t nq, int
     B2_TRY(idx->scalar.ensure(64));
     B2_TRY(launch_row_norms(q_dev, q_dtype, nq, X.d, idx->q_norm2.as<float>(), idx->scalar.as<float>() + 8, st));
     B2_TRY(launch_shard_lower_bound(idx->cand_score.as<float>(), idx->cand_id.as<int32_t>(), nq, 2 * c.n_splits, p.kp / 2, j,
-                                    idx->q_norm2.as<float>(), X.max_norm, p.rel_eps, idx->metric, lower_dev, st));
+                                    idx->q_norm2.as<float>(), X.max_norm, p.rel_eps, p.abs_eps, p.q_norm_limit, idx->metric, lower_dev, st));
     g_stats[ST_QUERIES] += nq;
     return B2_OK;
 }
@@ -704,6 +724,16 @@ int b2_debug_filter_lists(b2_index* idx, const void* q, int64_t nq, int32_t q_dt
     B2_CUDA(cudaMemcpyAsync(cand_thr, idx->cand_thr.p, (size_t)nq * c.n_splits * 2 * sizeof(float), cudaMemcpyDeviceToHost, st));
     cudaError_t e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) { set_error("filter failed on the device: %s", cudaGetErrorString(e)); return B2_ECUDA; }
+    return B2_OK;
+}
+
+int b2_debug_filter_eps(int32_t store_dtype, int32_t filt_dtype, int32_t q_dtype, int32_t d, float* rel_eps, float* abs_eps) {
+    if (!dtype_valid(store_dtype) || !dtype_valid(filt_dtype) || !dtype_valid(q_dtype) || d <= 0 || !rel_eps || !abs_eps) {
+        set_error("bad arguments");
+        return B2_EINVAL;
+    }
+    *rel_eps = filter_rel_eps(store_dtype, filt_dtype, q_dtype, d);
+    *abs_eps = filter_abs_eps(store_dtype, filt_dtype, q_dtype, d);
     return B2_OK;
 }
 

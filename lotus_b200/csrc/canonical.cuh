@@ -16,9 +16,21 @@ __device__ __forceinline__ double butterfly_sum(double v) {
     return v;
 }
 
-__device__ __forceinline__ float elem_f32(const void* base, int dtype, size_t i) {
-    return dtype == B2_F32 ? reinterpret_cast<const float*>(base)[i]
-                           : __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(base)[i]);
+// four 2-byte elements packed in a uint2 (element order = memory order), as fp32
+template <int DT>
+__device__ __forceinline__ void unpack4(const uint2& t, float (&o)[4]) {
+    static_assert(DT == B2_BF16 || DT == B2_F16, "2-byte element types only");
+    if constexpr (DT == B2_BF16) {  // the high half of a word is a bf16 value already aligned as fp32
+        o[0] = __uint_as_float(t.x << 16);
+        o[1] = __uint_as_float(t.x & 0xffff0000u);
+        o[2] = __uint_as_float(t.y << 16);
+        o[3] = __uint_as_float(t.y & 0xffff0000u);
+    } else {
+        o[0] = half_bits_f32<DT>(t.x & 0xffffu);
+        o[1] = half_bits_f32<DT>(t.x >> 16);
+        o[2] = half_bits_f32<DT>(t.y & 0xffffu);
+        o[3] = half_bits_f32<DT>(t.y >> 16);
+    }
 }
 
 // 4 consecutive elements of group g of a row (zero beyond d). `vec` = row start is 4-element aligned.
@@ -28,12 +40,10 @@ __device__ __forceinline__ void load_group(const void* row, int dtype, int g, in
         if (dtype == B2_F32) {
             const float4 t = __ldg(reinterpret_cast<const float4*>(row) + g);
             o[0] = t.x; o[1] = t.y; o[2] = t.z; o[3] = t.w;
-        } else {
-            const uint2 t = __ldg(reinterpret_cast<const uint2*>(row) + g);
-            o[0] = __uint_as_float(t.x << 16);
-            o[1] = __uint_as_float(t.x & 0xffff0000u);
-            o[2] = __uint_as_float(t.y << 16);
-            o[3] = __uint_as_float(t.y & 0xffff0000u);
+        } else if (dtype == B2_BF16) {
+            unpack4<B2_BF16>(__ldg(reinterpret_cast<const uint2*>(row) + g), o);
+        } else {  // B2_F16
+            unpack4<B2_F16>(__ldg(reinterpret_cast<const uint2*>(row) + g), o);
         }
     } else {
 #pragma unroll

@@ -1,6 +1,7 @@
 // common.cuh — shared declarations for libb2lotus.so (sm_90a only).
 #pragma once
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 
 #include <cfloat>
@@ -77,10 +78,43 @@ __host__ __device__ __forceinline__ float best_first_unkey(uint32_t k, int metri
     return f32_unord(metric == B2_METRIC_IP ? ~k : k);
 }
 
+// ---- element types -------------------------------------------------------------------------------------------
+// Every choice that depends on an element type goes through these helpers, so each of them names all three types.
+__host__ __device__ __forceinline__ bool dtype_valid(int dtype) { return dtype == B2_F32 || dtype == B2_BF16 || dtype == B2_F16; }
+__host__ __device__ constexpr int esize(int dtype) { return dtype == B2_F32 ? 4 : (dtype == B2_BF16 || dtype == B2_F16) ? 2 : 0; }
+// elements per 16 bytes: the row pitch of a TMA operand is a multiple of this
+__host__ __device__ constexpr int tma_align_elems(int dtype) { return 16 / esize(dtype); }
+
+// the fp32 value of the 2-byte pattern `h` (exact for both 2-byte types)
+template <int DT>
+__device__ __forceinline__ float half_bits_f32(uint32_t h) {
+    static_assert(DT == B2_BF16 || DT == B2_F16, "2-byte element types only");
+    if constexpr (DT == B2_BF16) return __uint_as_float(h << 16);
+    else return __half2float(__ushort_as_half((unsigned short)h));
+}
+
+// element i of a row-major matrix of `dtype`, as fp32 (exact)
+__device__ __forceinline__ float elem_f32(const void* base, int dtype, size_t i) {
+    switch (dtype) {
+        case B2_F32: return reinterpret_cast<const float*>(base)[i];
+        case B2_BF16: return __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(base)[i]);
+        default: return __half2float(reinterpret_cast<const __half*>(base)[i]);  // B2_F16
+    }
+}
+
+// out[i] = v rounded to nearest even in `dtype` (|v| >= 65520 becomes inf in fp16)
+__device__ __forceinline__ void store_elem(void* out, int dtype, size_t i, float v) {
+    switch (dtype) {
+        case B2_F32: reinterpret_cast<float*>(out)[i] = v; break;
+        case B2_BF16: reinterpret_cast<__nv_bfloat16*>(out)[i] = __float2bfloat16_rn(v); break;
+        default: reinterpret_cast<__half*>(out)[i] = __float2half_rn(v); break;  // B2_F16
+    }
+}
+
 // ---- a matrix the kernels can search ---------------------------------------------------------------------
-// `store` holds the exact values (dtype f32 or bf16, row pitch `d`). `filt` is what the wgmma filter
-// streams through TMA: bf16 (pitch multiple of 8 elements) for a bf16 index, fp32 (pitch multiple of 4)
-// read as TF32 for an fp32 index; it aliases `store` whenever the pitch already qualifies.
+// `store` holds the exact values (dtype f32, bf16 or f16, row pitch `d`). `filt` is what the wgmma filter
+// streams through TMA: the stored 2-byte values (pitch multiple of 8 elements) for a bf16 or fp16 index, fp32 (pitch
+// multiple of 4) read as TF32 for an fp32 index; it aliases `store` whenever the pitch already qualifies.
 struct MatView {
     const void* store = nullptr;
     const void* filt = nullptr;
@@ -88,7 +122,7 @@ struct MatView {
     int64_t n = 0;
     int32_t d = 0;
     int32_t dtype = B2_F32;       // element type of `store`
-    int32_t filt_dtype = B2_F32;  // element type of `filt`: B2_BF16 -> bf16 wgmma, B2_F32 -> tf32 wgmma
+    int32_t filt_dtype = B2_F32;  // element type of `filt`: B2_BF16 -> bf16 wgmma, B2_F16 -> fp16 wgmma, B2_F32 -> tf32 wgmma
     int64_t filt_pitch = 0;  // elements
     // fp32 stores only (optional): a bf16 rounding of the rows, pitch multiple of 8. When present, searches run a FIRST level on it
     // (bf16 wgmma at twice the tf32 rate, operand error 2^-8 per fp32 operand in the certificate) and only the queries whose
@@ -127,11 +161,11 @@ int launch_gather_rows(const void* x, int dtype, int d, const int64_t* ids, int6
                        int* err_flag, cudaStream_t stream);
 int launch_finalize(const MatView& X, const void* q, int q_dtype, int64_t nq, int metric, int k, int kp, int list_len,
                     int n_lists, const float* cand_score, const int32_t* cand_id, const float* cand_thr,
-                    float rel_eps, const int64_t* id_map, int64_t id_offset, float* out_scores, int64_t* out_idx,
-                    int32_t* flags, int32_t* sel, int32_t* sel_count, cudaStream_t stream, const float* hint = nullptr);
+                    float rel_eps, float abs_eps, float q_norm_limit, const int64_t* id_map, int64_t id_offset, float* out_scores,
+                    int64_t* out_idx, int32_t* flags, int32_t* sel, int32_t* sel_count, cudaStream_t stream, const float* hint = nullptr);
 int shard_lower_bound_max_entries();
 int launch_shard_lower_bound(const float* cand_score, const int32_t* cand_id, int64_t nq, int n_lists, int list_len, int j, const float* qnorm2,
-                             float max_norm, float rel_eps, int metric, float* lower, cudaStream_t stream);
+                             float max_norm, float rel_eps, float abs_eps, float q_norm_limit, int metric, float* lower, cudaStream_t stream);
 int launch_fill_f32(float* p, int64_t n, float v, cudaStream_t stream);
 int launch_dense_topk(const MatView& X, const void* q, int q_dtype, int64_t nq, const int32_t* q_sel,
                       int64_t n_sel, int metric, int k, const int64_t* id_map, int64_t id_offset, float* dense_ws,

@@ -7,36 +7,11 @@
 #include <algorithm>
 #include <vector>
 
+#include "canonical.cuh"
 #include "index.cuh"
 
 namespace b2 {
 namespace {
-
-constexpr unsigned FULL = 0xffffffffu;
-
-__device__ __forceinline__ void load_group2(const char* row, int dtype, int g, int d, bool vec, float (&o)[4]) {
-    const int i0 = g * 4;
-    if (vec) {
-        if (dtype == B2_F32) {
-            const float4 t = __ldg(reinterpret_cast<const float4*>(row) + g);
-            o[0] = t.x; o[1] = t.y; o[2] = t.z; o[3] = t.w;
-        } else {
-            const uint2 t = __ldg(reinterpret_cast<const uint2*>(row) + g);
-            o[0] = __uint_as_float(t.x << 16);
-            o[1] = __uint_as_float(t.x & 0xffff0000u);
-            o[2] = __uint_as_float(t.y << 16);
-            o[3] = __uint_as_float(t.y & 0xffff0000u);
-        }
-    } else {
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-            const int i = i0 + e;
-            o[e] = i < d ? (dtype == B2_F32 ? reinterpret_cast<const float*>(row)[i]
-                                            : __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(row)[i]))
-                         : 0.f;
-        }
-    }
-}
 
 // one warp per candidate pair: canonical inner product (same order as oracle orc_dot_canonical), strict compare
 __global__ void pair_verify_kernel(const char* store, int dtype, int d, const int32_t* ci, const int32_t* cj, int64_t ncand,
@@ -45,7 +20,7 @@ __global__ void pair_verify_kernel(const char* store, int dtype, int d, const in
     const int64_t warp = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
     const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
     const bool vec = (d % 4) == 0;
-    const size_t row_bytes = (size_t)d * (dtype == B2_F32 ? 4 : 2);
+    const size_t row_bytes = (size_t)d * esize(dtype);
     const int ngroups = (d + 3) >> 2;
     for (int64_t c = warp; c < ncand; c += nwarps) {
         const int i = ci[c], j = cj[c];
@@ -54,8 +29,8 @@ __global__ void pair_verify_kernel(const char* store, int dtype, int d, const in
         double acc = 0.0;
         for (int g = lane; g < ngroups; g += 32) {
             float a[4], b[4];
-            load_group2(ri, dtype, g, d, vec, a);
-            load_group2(rj, dtype, g, d, vec, b);
+            load_group(ri, dtype, g, d, vec, a);
+            load_group(rj, dtype, g, d, vec, b);
 #pragma unroll
             for (int e = 0; e < 4; ++e) acc = fma((double)a[e], (double)b[e], acc);
         }

@@ -110,7 +110,12 @@ struct FilterPlan {
     std::vector<FilterChunk> chunks;
     int64_t q_pitch = 0;
     bool q_in_place = false;  // the queries already have the filter's type and a TMA-compatible pitch
+    // |filter score - exact <q, x>| <= rel_eps |q| |x| + abs_eps (|q| + |x|) (filter_rel_eps / filter_abs_eps)
     float rel_eps = 0.f;
+    float abs_eps = 0.f;
+    // a query whose norm reaches this is not certified from its lists: fp32 / bf16 queries rounded to fp16 for the filter
+    // overflow to inf from a component of 65520 on, and such a component makes the norm at least that large
+    float q_norm_limit = INFINITY;
 };
 
 }  // namespace b2
@@ -146,8 +151,6 @@ struct b2_index {
 
 namespace b2 {
 
-static inline size_t esize(int dtype) { return dtype == B2_F32 ? 4 : 2; }
-
 // searchable view (filter operand, row norms, max norm) of a row-major device matrix
 int build_view(const void* store, int64_t n, int d, int dtype, DevBuf& filt_pad, DevBuf& norm2, DevBuf& scalar, MatView& v,
                cudaStream_t st, DevBuf* filt16 = nullptr);
@@ -155,6 +158,7 @@ int build_view(const void* store, int64_t n, int d, int dtype, DevBuf& filt_pad,
 int search_core(b2_index* idx, const MatView& X, int metric, const void* q_dev, int q_dtype, int64_t nq, int k,
                 const int64_t* id_map, int64_t id_offset, float* out_sc, int64_t* out_id, cudaStream_t st, int level = 0);
 float filter_rel_eps(int store_dtype, int filt_dtype, int q_dtype, int d);
+float filter_abs_eps(int store_dtype, int filt_dtype, int q_dtype, int d);
 int plan_filter(const MatView& X, const void* q, int q_dtype, int64_t nq, int k, bool top1, int num_sms, FilterPlan& plan);
 // prep one chunk's queries (unless streamed in place), size the candidate workspace and run the filter between idx->ev0 and ev1
 int run_filter(b2_index* idx, const FilterPlan& plan, const FilterChunk& c, int metric, cudaStream_t st);

@@ -125,8 +125,7 @@ __global__ void prep_queries_kernel(const void* q, int q_dtype, int64_t nq, int 
         const int64_t r = t / pitch;
         const int c = (int)(t - r * pitch);
         const float v = c < d ? elem_f32(q, q_dtype, (size_t)(r * d + c)) : 0.f;
-        if (out_dtype == B2_F32) reinterpret_cast<float*>(out)[t] = v;
-        else reinterpret_cast<__nv_bfloat16*>(out)[t] = __float2bfloat16_rn(v);
+        store_elem(out, out_dtype, (size_t)t, v);
     }
 }
 
@@ -135,7 +134,7 @@ __global__ void row_norms_kernel(const void* x, int dtype, int64_t n, int d, flo
     const int64_t warp = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
     const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
     const bool vec = (d % 4) == 0;
-    const size_t esz = dtype == B2_F32 ? 4 : 2;
+    const size_t esz = esize(dtype);
     float local_max = 0.f;
     for (int64_t j = warp; j < n; j += nwarps) {
         const char* row = reinterpret_cast<const char*>(x) + (size_t)j * d * esz;
@@ -160,8 +159,7 @@ __global__ void convert_pad_kernel(const void* x, int dtype, int64_t n, int d, v
         const int64_t r = t / pitch;
         const int c = (int)(t - r * pitch);
         const float v = c < d ? elem_f32(x, dtype, (size_t)(r * d + c)) : 0.f;
-        if (out_dtype == B2_F32) reinterpret_cast<float*>(out)[t] = v;
-        else reinterpret_cast<__nv_bfloat16*>(out)[t] = __float2bfloat16_rn(v);
+        store_elem(out, out_dtype, (size_t)t, v);
     }
 }
 
@@ -193,7 +191,7 @@ __global__ void gather_rows_kernel(const char* x, size_t row_bytes, const int64_
 
 // Canonical partials of U rows at once (vectorisable rows only): the U independent row loads of a step are issued
 // back to back, so each lane keeps U gathers in flight. Per row the accumulation order is exactly canonical_partial's.
-template <bool IS_L2, bool BF16, int U>
+template <bool IS_L2, int DT, int U>
 __device__ __forceinline__ void canonical_partial_multi(const float* q_s, const char* const (&rows)[U], int d, int lane,
                                                         double (&acc)[U]) {
 #pragma unroll
@@ -201,17 +199,12 @@ __device__ __forceinline__ void canonical_partial_multi(const float* q_s, const 
     const int ngroups = d >> 2;
     for (int g = lane; g < ngroups; g += 32) {
         float x[U][4];
-        if constexpr (BF16) {
+        if constexpr (DT != B2_F32) {  // B2_BF16, B2_F16
             uint2 t[U];
 #pragma unroll
             for (int u = 0; u < U; ++u) t[u] = __ldg(reinterpret_cast<const uint2*>(rows[u]) + g);
 #pragma unroll
-            for (int u = 0; u < U; ++u) {
-                x[u][0] = __uint_as_float(t[u].x << 16);
-                x[u][1] = __uint_as_float(t[u].x & 0xffff0000u);
-                x[u][2] = __uint_as_float(t[u].y << 16);
-                x[u][3] = __uint_as_float(t[u].y & 0xffff0000u);
-            }
+            for (int u = 0; u < U; ++u) unpack4<DT>(t[u], x[u]);
         } else {
             float4 t[U];
 #pragma unroll
@@ -255,7 +248,8 @@ struct FinalizeParams {
     int64_t id_offset;
     int32_t d, dtype, q_dtype, metric, k, kp, n_splits;  // n_splits = number of candidate lists per query, kp = survivors kept
     int32_t list_len;                                    // entries per candidate list (<= 32*R)
-    float rel_eps, max_norm;
+    float rel_eps, abs_eps, max_norm;
+    float q_norm_limit;         // queries with |q| >= this are not certified (fp16-rounded filter operand may overflow)
     const float* max_norm_dev;  // nullable: overrides max_norm
     const float* hint;          // nullable: per query, a lower bound (filter-score space) on the k-th exact score of the WHOLE
                                 // row-sharded search (b2_index_search_stage1_dev + all-reduce MIN over the ranks)
@@ -281,7 +275,7 @@ __global__ void __launch_bounds__(FIN_WARPS * 32) finalize_kernel(const Finalize
     const float max_norm = p.max_norm_dev ? __ldg(p.max_norm_dev) : p.max_norm;
     const bool is_l2 = p.metric == B2_METRIC_L2;
     const bool vec = (p.d % 4) == 0;
-    const size_t esz = p.dtype == B2_F32 ? 4 : 2;
+    const size_t esz = esize(p.dtype);
 
     // 1. query -> smem (fp32, exact upcast for bf16) and its canonical squared norm
     for (int i = lane; i < d4; i += 32) q_s[i] = i < p.d ? elem_f32(p.q, p.q_dtype, (size_t)q * p.d + i) : 0.f;
@@ -339,8 +333,10 @@ __global__ void __launch_bounds__(FIN_WARPS * 32) finalize_kernel(const Finalize
     }
     // margin between a filter score and the exact score it stands for (same quantity the certificate uses below)
     const double qn_m = sqrt(qn2), mx_m = (double)max_norm;
-    const double eps_f = is_l2 ? 2.0 * (double)p.rel_eps * qn_m * mx_m + 2.4e-7 * (mx_m * mx_m + 2.0 * qn_m * mx_m) + 1e-30
-                               : (double)p.rel_eps * qn_m * mx_m + 1e-30;
+    // (the absolute term is zero unless an operand was rounded to fp16; adding it last keeps the other margins bit for bit)
+    const double eps_f = is_l2 ? 2.0 * (double)p.rel_eps * qn_m * mx_m + 2.4e-7 * (mx_m * mx_m + 2.0 * qn_m * mx_m) + 1e-30 +
+                                     2.0 * (double)p.abs_eps * (qn_m + mx_m)
+                               : (double)p.rel_eps * qn_m * mx_m + 1e-30 + (double)p.abs_eps * (qn_m + mx_m);
     // Pruning before the (expensive) re-score: the k best survivors BY FILTER SCORE have exact scores >= t_k - eps, so a
     // survivor whose filter score is below t_k - 2 eps is strictly worse than k others: it cannot enter or tie the top k.
 #pragma unroll
@@ -385,11 +381,14 @@ __global__ void __launch_bounds__(FIN_WARPS * 32) finalize_kernel(const Finalize
             for (int u = 0; u < 4; ++u)
                 rows[u] = reinterpret_cast<const char*>(p.store) + (size_t)(ids[u] >= 0 ? ids[u] : ids[0]) * p.d * esz;
             if (p.dtype == B2_BF16) {
-                if (is_l2) canonical_partial_multi<true, true, 4>(q_s, rows, p.d, lane, part);
-                else canonical_partial_multi<false, true, 4>(q_s, rows, p.d, lane, part);
-            } else {
-                if (is_l2) canonical_partial_multi<true, false, 4>(q_s, rows, p.d, lane, part);
-                else canonical_partial_multi<false, false, 4>(q_s, rows, p.d, lane, part);
+                if (is_l2) canonical_partial_multi<true, B2_BF16, 4>(q_s, rows, p.d, lane, part);
+                else canonical_partial_multi<false, B2_BF16, 4>(q_s, rows, p.d, lane, part);
+            } else if (p.dtype == B2_F16) {
+                if (is_l2) canonical_partial_multi<true, B2_F16, 4>(q_s, rows, p.d, lane, part);
+                else canonical_partial_multi<false, B2_F16, 4>(q_s, rows, p.d, lane, part);
+            } else {  // B2_F32
+                if (is_l2) canonical_partial_multi<true, B2_F32, 4>(q_s, rows, p.d, lane, part);
+                else canonical_partial_multi<false, B2_F32, 4>(q_s, rows, p.d, lane, part);
             }
         } else {
 #pragma unroll
@@ -484,16 +483,20 @@ __global__ void __launch_bounds__(FIN_WARPS * 32) finalize_kernel(const Finalize
             const double qn = sqrt(qn2);
             const double v = (double)best_first_unkey((uint32_t)(s_keys[k - 1] >> 32), p.metric);
             if (!is_l2) {
-                const double eps = (double)p.rel_eps * qn * (double)max_norm + 1e-30;
+                const double eps = (double)p.rel_eps * qn * (double)max_norm + 1e-30 + (double)p.abs_eps * (qn + (double)max_norm);
                 certified = ((double)bound + eps) < v;
             } else {
                 const double mx = (double)max_norm;
-                const double eps_s = 2.0 * (double)p.rel_eps * qn * mx + 2.4e-7 * (mx * mx + 2.0 * qn * mx) + 1e-30;
+                const double eps_s = 2.0 * (double)p.rel_eps * qn * mx + 2.4e-7 * (mx * mx + 2.0 * qn * mx) + 1e-30 +
+                                     2.0 * (double)p.abs_eps * (qn + mx);
                 // discarded rows have exact L2 >= qn2 - (bound + eps_s); allow for the fp32 rounding of v
                 certified = (qn2 - (double)bound - eps_s) > v * (1.0 + 2.4e-7) + 1e-30;
             }
         }
     }
+
+    // a query that may have overflowed when it was rounded for the filter: its lists prove nothing
+    if (p.q_norm_limit < INFINITY && !(qn2 < (double)p.q_norm_limit * (double)p.q_norm_limit)) certified = false;
 
     // 7. write
     const float pad = is_l2 ? FLT_MAX : -FLT_MAX;
@@ -526,7 +529,7 @@ __global__ void dense_scores_kernel(const void* store, int dtype, int64_t n, int
     const int lane = threadIdx.x & 31;
     const int d4 = ((d + 3) >> 2) << 2;
     const bool vec = (d % 4) == 0;
-    const size_t esz = dtype == B2_F32 ? 4 : 2;
+    const size_t esz = esize(dtype);
     const bool is_l2 = metric == B2_METRIC_L2;
     const int64_t warp = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
     const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
@@ -825,7 +828,8 @@ __global__ void exact_l2_assigned_kernel(const void* pts, int dtype, int64_t m, 
 // the index are known to score at least that much. Warp per query; up to 32 * LB_R candidate entries.
 constexpr int LB_R = 32;
 __global__ void shard_lower_bound_kernel(const float* cand_score, const int32_t* cand_id, int64_t nq, int n_lists, int list_len, int j,
-                                         const float* qnorm2, float max_norm, float rel_eps, int metric, float* lower) {
+                                         const float* qnorm2, float max_norm, float rel_eps, float abs_eps, float q_norm_limit, int metric,
+                                         float* lower) {
     const int lane = threadIdx.x & 31;
     const int64_t q = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
     if (q >= nq) return;
@@ -864,10 +868,12 @@ __global__ void shard_lower_bound_kernel(const float* cand_score, const int32_t*
     }
     if (lane == 0) {
         float out = -INFINITY;
-        if (tj > -INFINITY) {
-            const double qn = sqrt((double)qnorm2[q]), mx = (double)max_norm;
-            const double eps = metric == B2_METRIC_L2 ? 2.0 * (double)rel_eps * qn * mx + 2.4e-7 * (mx * mx + 2.0 * qn * mx) + 1.3e-7 * qn * qn + 1e-30
-                                                      : (double)rel_eps * qn * mx * (1.0 + 1.3e-7) + 1e-30;
+        const double qn = sqrt((double)qnorm2[q]), mx = (double)max_norm;
+        // (qnorm2 is the fp32 rounding of |q|^2: q_norm_limit = 65504 is below the overflow threshold 65520 by more than that)
+        if (tj > -INFINITY && (q_norm_limit == INFINITY || qn < (double)q_norm_limit)) {
+            const double eps = metric == B2_METRIC_L2 ? 2.0 * (double)rel_eps * qn * mx + 2.4e-7 * (mx * mx + 2.0 * qn * mx) + 1.3e-7 * qn * qn + 1e-30 +
+                                                            2.0 * (double)abs_eps * (qn + mx) * (1.0 + 1.3e-7)
+                                                      : (double)rel_eps * qn * mx * (1.0 + 1.3e-7) + 1e-30 + (double)abs_eps * (qn + mx) * (1.0 + 1.3e-7);
             out = (float)((double)tj - eps - 4.8e-7 * fabs((double)tj));
         }
         lower[q] = out;
@@ -908,10 +914,10 @@ int launch_row_norms(const void* x, int dtype, int64_t n, int d, float* norm2, f
 int shard_lower_bound_max_entries() { return 32 * LB_R; }
 
 int launch_shard_lower_bound(const float* cand_score, const int32_t* cand_id, int64_t nq, int n_lists, int list_len, int j, const float* qnorm2,
-                             float max_norm, float rel_eps, int metric, float* lower, cudaStream_t stream) {
+                             float max_norm, float rel_eps, float abs_eps, float q_norm_limit, int metric, float* lower, cudaStream_t stream) {
     if (nq <= 0) return B2_OK;
     shard_lower_bound_kernel<<<(unsigned)ceil_div(nq * 32, 128), 128, 0, stream>>>(cand_score, cand_id, nq, n_lists, list_len, j, qnorm2, max_norm,
-                                                                                  rel_eps, metric, lower);
+                                                                                  rel_eps, abs_eps, q_norm_limit, metric, lower);
     B2_LAUNCH_CHECK();
     return B2_OK;
 }
@@ -949,7 +955,7 @@ int launch_convert_pad(const void* x, int dtype, int64_t n, int d, void* out, in
 int launch_gather_rows(const void* x, int dtype, int d, const int64_t* ids, int64_t m, int64_t n, void* out,
                        int* err_flag, cudaStream_t stream) {
     if (m <= 0) return B2_OK;
-    const size_t row_bytes = (size_t)d * (dtype == B2_F32 ? 4 : 2);
+    const size_t row_bytes = (size_t)d * esize(dtype);
     gather_rows_kernel<<<grid_for(m * 32, 256), 256, 0, stream>>>(reinterpret_cast<const char*>(x), row_bytes, ids, m, n,
                                                                   reinterpret_cast<char*>(out), err_flag);
     B2_LAUNCH_CHECK();
@@ -975,8 +981,8 @@ static int launch_finalize_r(const FinalizeParams& p, cudaStream_t stream) {
 
 int launch_finalize(const MatView& X, const void* q, int q_dtype, int64_t nq, int metric, int k, int kp, int list_len,
                     int n_splits, const float* cand_score, const int32_t* cand_id, const float* cand_thr,
-                    float rel_eps, const int64_t* id_map, int64_t id_offset, float* out_scores, int64_t* out_idx,
-                    int32_t* flags, int32_t* sel, int32_t* sel_count, cudaStream_t stream, const float* hint) {
+                    float rel_eps, float abs_eps, float q_norm_limit, const int64_t* id_map, int64_t id_offset, float* out_scores,
+                    int64_t* out_idx, int32_t* flags, int32_t* sel, int32_t* sel_count, cudaStream_t stream, const float* hint) {
     if (nq <= 0) return B2_OK;
     FinalizeParams p;
     p.hint = hint;
@@ -1002,6 +1008,8 @@ int launch_finalize(const MatView& X, const void* q, int q_dtype, int64_t nq, in
     p.list_len = list_len;
     p.n_splits = n_splits;
     p.rel_eps = rel_eps;
+    p.abs_eps = abs_eps;
+    p.q_norm_limit = q_norm_limit;
     p.max_norm = X.max_norm;
     p.max_norm_dev = X.max_norm_dev;
     g_stats[ST_RESCORED] += nq * (int64_t)kp;
@@ -1055,7 +1063,7 @@ int launch_dense_topk(const MatView& X, const void* q, int q_dtype, int64_t nq, 
         const int sc = (int)std::min<int64_t>(dense_ws_rows, n_sel - s0);
         const int32_t* sel = q_sel ? q_sel + s0 : nullptr;
         // without a selection list the batch is the contiguous query range [s0, s0+sc)
-        const void* qb = q_sel ? q : reinterpret_cast<const char*>(q) + (size_t)s0 * X.d * (q_dtype == B2_F32 ? 4 : 2);
+        const void* qb = q_sel ? q : reinterpret_cast<const char*>(q) + (size_t)s0 * X.d * esize(q_dtype);
         if (X.n > 0) {
             dense_scores_kernel<<<grid_for(X.n * 32, 256, 132 * 8), 256, smem, stream>>>(X.store, X.dtype, X.n, X.d, qb, q_dtype,
                                                                                        sel, sc, metric, dense_ws);

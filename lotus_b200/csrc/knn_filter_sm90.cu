@@ -5,7 +5,7 @@
 // (knn_inner_product / knn_L2sqr: blocked sgemm + heap). The N x Q score matrix is never written to HBM.
 //
 // Role of this kernel in the exact pipeline (DESIGN.md §Pipeline): it is a FILTER. It computes scores with
-// bf16 (or TF32) tensor-core products and fp32 accumulation and keeps, per query and per corpus split,
+// bf16 / fp16 (or TF32) tensor-core products and fp32 accumulation and keeps, per query and per corpus split,
 // the KP > k best candidates plus the value `thr` below which everything was discarded. knn_exact.cu then
 // re-scores the candidates in the canonical fp64 order and certifies, with a rigorous error margin, that
 // nothing discarded could belong to the true top-k; uncertified queries take the dense exact path.
@@ -14,7 +14,7 @@
 //   warpgroup 0: TMA producer (one lane)
 //   warpgroups 1, 2: consumers; consumer g issues wgmma m64n256 for query rows 64g..64g+63 (fp32 accumulators in
 //                    registers, 128 per thread) and runs the epilogue of those rows
-//   K-block = one 64-byte swizzle row (32 bf16 / 16 tf32): wgmma k16 (bf16) or k8 (tf32), two per K-block.
+//   K-block = one 64-byte swizzle row (32 bf16 or fp16 / 16 tf32): wgmma k16 (bf16, fp16) or k8 (tf32), two per K-block.
 //   smem ring of NSTAGES x (A 8 KB + B 16 KB), mbarrier full/empty pairs.
 //   CTA pairs (default once there are two query tiles): a 2-CTA cluster takes two consecutive query tiles and sweeps the
 //   same corpus tiles; each CTA loads HALF of every corpus tile and TMA-multicasts it into both CTAs, so the corpus bytes
@@ -185,25 +185,30 @@ __device__ __forceinline__ void acc_fence(float (&d)[128]) {
     for (int i = 0; i < 128; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
+// Operand kind of the filter: the element type both wgmma operands are streamed in. BF16 and F16 are 2-byte operands
+// (m64n256k16, 32 elements per K-block); TF32 reads fp32 operands (m64n256k8, 16 elements per K-block).
+enum class Op { BF16, F16, TF32 };
+__host__ __device__ constexpr int op_bytes(Op op) { return op == Op::TF32 ? 4 : 2; }
+
+#define B2_WGMMA_64X256(SHAPE_TYPES, IMM_TAIL)                                                                               \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"                                                   \
+                 "wgmma.mma_async.sync.aligned." SHAPE_TYPES " "                                                           \
+                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}" ", %128, %129, p, 1, 1" IMM_TAIL ";\n\t}"                                                          \
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])                                                                                                         \
+                 : "l"(adesc), "l"(bdesc), "r"(scale_d))
+
 // D[64 x 256] (+)= A[64 x K] . B[256 x K]^T, both K-major in shared memory; scale_d == 0 overwrites D
-template <bool TF32>
+template <Op OP>
 __device__ __forceinline__ void wgmma_64x256(float (&d)[128], uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
-    if constexpr (TF32) {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
-            "wgmma.mma_async.sync.aligned.m64n256k8.f32.tf32.tf32 "
-            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1;\n\t}"
-            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
-            : "l"(adesc), "l"(bdesc), "r"(scale_d));
-    } else {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
-            "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 "
-            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1, 0, 0;\n\t}"
-            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
-            : "l"(adesc), "l"(bdesc), "r"(scale_d));
+    if constexpr (OP == Op::TF32) {
+        B2_WGMMA_64X256("m64n256k8.f32.tf32.tf32", "");
+    } else if constexpr (OP == Op::F16) {
+        B2_WGMMA_64X256("m64n256k16.f32.f16.f16", ", 0, 0");
+    } else {  // Op::BF16
+        B2_WGMMA_64X256("m64n256k16.f32.bf16.bf16", ", 0, 0");
     }
 }
+#undef B2_WGMMA_64X256
 
 struct FilterParams {
     const float* xnorm;  // [n], L2 only
@@ -298,10 +303,10 @@ __device__ __forceinline__ void item_range(const FilterParams& p, const Sched& s
 
 // TMA producer: one lane (per CTA) streams (query tile, corpus tile) K-blocks into the smem ring. In a CTA pair each CTA
 // loads its own query rows and half of the corpus tile, multicast to both CTAs; every CTA's full barrier counts a whole stage.
-template <bool TF32, int NSTAGES, bool TWO>
+template <Op OP, int NSTAGES, bool TWO>
 __device__ __forceinline__ void producer_loop(const CUtensorMap* tmap_q, const CUtensorMap* tmap_x, const FilterParams& p,
                                               const Ring& r, const Sched& sc) {
-    constexpr int KB_ELEMS = KB_BYTES / (TF32 ? 4 : 2);
+    constexpr int KB_ELEMS = KB_BYTES / op_bytes(OP);
     const int n_items = num_items(p);
     int stage = 0;
     uint32_t phase = 0;
@@ -341,7 +346,7 @@ __device__ __forceinline__ void release_stage(const Ring& r, int s, int rank) {
 
 // Consumer warpgroup g: acc = (query rows 64g..64g+63 of the stage's A tile) . (the 256 corpus rows)^T over all K-blocks of
 // one corpus tile. One wgmma group per K-block; a stage is released as soon as the group that read it has retired.
-template <bool TF32, int NSTAGES, bool TWO>
+template <Op OP, int NSTAGES, bool TWO>
 __device__ __forceinline__ void mma_tile(float (&acc)[128], const Ring& r, int num_kb, int g, int rank, int& stage, uint32_t& phase) {
     const uint32_t a_off = (uint32_t)(g * WG_M * KB_BYTES);
     int prev = -1;
@@ -353,7 +358,7 @@ __device__ __forceinline__ void mma_tile(float (&acc)[128], const Ring& r, int n
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < KSTEPS; ++k)  // +32 bytes per K step inside the 64-byte swizzle row (16 B units)
-            wgmma_64x256<TF32>(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (kb | k) != 0 ? 1u : 0u);
+            wgmma_64x256<OP>(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (kb | k) != 0 ? 1u : 0u);
         wgmma_commit();
         if (prev >= 0) {
             wgmma_wait<1>();
@@ -517,7 +522,7 @@ __device__ __forceinline__ void process8_top2(const float (&v)[8], int idx0, flo
     }
 }
 
-template <int KP, bool IS_L2, bool TF32, bool TWO, bool TOP1 = false>
+template <int KP, bool IS_L2, Op OP, bool TWO, bool TOP1 = false>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 knn_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_x,
                   const FilterParams p) {
@@ -542,7 +547,7 @@ knn_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
 
     if (warp < 4) {
         setmaxnreg_dec<40>();
-        if (threadIdx.x == 0) producer_loop<TF32, NSTAGES, TWO>(&tmap_q, &tmap_x, p, ring, sc);
+        if (threadIdx.x == 0) producer_loop<OP, NSTAGES, TWO>(&tmap_q, &tmap_x, p, ring, sc);
     } else {
         setmaxnreg_inc<232>();
         // ===================== consumer warpgroup g: wgmma of 64 query rows, streaming top-KPH per (row, set) ==========
@@ -579,7 +584,7 @@ knn_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
             // lane fr + 8h + 16s
             float gthr[2][2] = {{-INFINITY, -INFINITY}, {-INFINITY, -INFINITY}};
             for (int t = t0; t < t1; ++t) {
-                mma_tile<TF32, NSTAGES, TWO>(acc, ring, p.num_kb, g, sc.rank, stage, phase);
+                mma_tile<OP, NSTAGES, TWO>(acc, ring, p.num_kb, g, sc.rank, stage, phase);
                 const int col0 = t * BLOCK_N;
                 const int ncols = min(BLOCK_N, p.n - col0);
 #pragma unroll
@@ -674,7 +679,7 @@ knn_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
 constexpr int PAIR_STAGES = MAX_STAGES;
 constexpr int PAIR_SMEM = PAIR_STAGES * STAGE_BYTES + BAR_BYTES + SMEM_ALIGN_SLACK;
 
-template <bool TF32, bool TWO>
+template <Op OP, bool TWO>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 pair_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_x, const FilterParams p) {
     extern __shared__ uint8_t smem_raw[];
@@ -686,7 +691,7 @@ pair_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_cons
     const Sched sc = make_sched<TWO>();
     if (warp < 4) {
         setmaxnreg_dec<40>();
-        if (threadIdx.x == 0) producer_loop<TF32, PAIR_STAGES, TWO>(&tmap_q, &tmap_x, p, ring, sc);
+        if (threadIdx.x == 0) producer_loop<OP, PAIR_STAGES, TWO>(&tmap_q, &tmap_x, p, ring, sc);
     } else {
         setmaxnreg_inc<232>();
         const int g = (warp >> 2) - 1;
@@ -700,7 +705,7 @@ pair_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_cons
             item_range<TWO>(p, sc, item, m_tile, split, t0, t1);
             const int gi0 = m_tile * BLOCK_M + g * WG_M + wq * 16 + (lane >> 2);  // global rows gi0 and gi0 + 8 of this lane
             for (int t = t0; t < t1; ++t) {
-                mma_tile<TF32, PAIR_STAGES, TWO>(acc, ring, p.num_kb, g, sc.rank, stage, phase);
+                mma_tile<OP, PAIR_STAGES, TWO>(acc, ring, p.num_kb, g, sc.rank, stage, phase);
                 const int col0 = t * BLOCK_N + 2 * (lane & 3);
                 float mx = acc[0];
 #pragma unroll
@@ -744,11 +749,27 @@ PFN_encodeTiled get_encode_fn() {
     return fn;
 }
 
+// the filter operand kind of a filter copy of `filt_dtype` elements
+Op filter_op(int filt_dtype) {
+    switch (filt_dtype) {
+        case B2_F32: return Op::TF32;
+        case B2_BF16: return Op::BF16;
+        default: return Op::F16;  // B2_F16
+    }
+}
+CUtensorMapDataType tma_data_type(Op op) {
+    switch (op) {
+        case Op::TF32: return CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+        case Op::BF16: return CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+        default: return CU_TENSOR_MAP_DATA_TYPE_FLOAT16;  // Op::F16
+    }
+}
+
 // 2-D row-major matrix [rows, cols] with `pitch` elements per row; box = {KB_BYTES of K, box_rows rows}
-int make_tmap(CUtensorMap* map, const void* base, bool tf32, int64_t rows, int64_t cols, int64_t pitch, int box_rows) {
+int make_tmap(CUtensorMap* map, const void* base, Op op, int64_t rows, int64_t cols, int64_t pitch, int box_rows) {
     PFN_encodeTiled enc = get_encode_fn();
     if (!enc) return B2_ECUDA;
-    const int esz = tf32 ? 4 : 2;
+    const int esz = op_bytes(op);
     cuuint64_t gdim[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
     cuuint64_t gstride[1] = {(cuuint64_t)pitch * esz};
     cuuint32_t box[2] = {(cuuint32_t)(KB_BYTES / esz), (cuuint32_t)box_rows};
@@ -757,7 +778,7 @@ int make_tmap(CUtensorMap* map, const void* base, bool tf32, int64_t rows, int64
         set_error("TMA operand not 16-byte aligned (base %p, pitch %lld B)", base, (long long)gstride[0]);
         return B2_EINVAL;
     }
-    CUresult r = enc(map, tf32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2,
+    CUresult r = enc(map, tma_data_type(op), 2,
                      const_cast<void*>(base), gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                      CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) {
@@ -792,40 +813,40 @@ int launch_cluster(Kern kern, int grid, int smem, bool two, const CUtensorMap& t
     return B2_OK;
 }
 
-template <int KP, bool IS_L2, bool TF32, bool TWO, bool TOP1 = false>
+template <int KP, bool IS_L2, Op OP, bool TWO, bool TOP1 = false>
 int launch_variant(const CUtensorMap& tq, const CUtensorMap& tx, const FilterParams& p, int grid, cudaStream_t stream) {
-    return launch_cluster(knn_filter_kernel<KP, IS_L2, TF32, TWO, TOP1>, grid, smem_bytes(KP), TWO, tq, tx, p, stream);
+    return launch_cluster(knn_filter_kernel<KP, IS_L2, OP, TWO, TOP1>, grid, smem_bytes(KP), TWO, tq, tx, p, stream);
+}
+
+template <int KP, bool IS_L2, bool TWO, bool TOP1 = false>
+int launch_op(Op op, const CUtensorMap& tq, const CUtensorMap& tx, const FilterParams& p, int grid, cudaStream_t stream) {
+    switch (op) {
+        case Op::TF32: return launch_variant<KP, IS_L2, Op::TF32, TWO, TOP1>(tq, tx, p, grid, stream);
+        case Op::BF16: return launch_variant<KP, IS_L2, Op::BF16, TWO, TOP1>(tq, tx, p, grid, stream);
+        default: return launch_variant<KP, IS_L2, Op::F16, TWO, TOP1>(tq, tx, p, grid, stream);  // Op::F16
+    }
 }
 
 template <int KP, bool TWO>
-int launch_kp(bool is_l2, bool tf32, const CUtensorMap& tq, const CUtensorMap& tx, const FilterParams& p, int grid,
+int launch_kp(bool is_l2, Op op, const CUtensorMap& tq, const CUtensorMap& tx, const FilterParams& p, int grid,
               cudaStream_t stream) {
     if constexpr (KP == 16) {
         if (p.top1) {  // k == 1: register-resident top-2 epilogue
-            if (is_l2) {
-                return tf32 ? launch_variant<KP, true, true, TWO, true>(tq, tx, p, grid, stream)
-                            : launch_variant<KP, true, false, TWO, true>(tq, tx, p, grid, stream);
-            }
-            return tf32 ? launch_variant<KP, false, true, TWO, true>(tq, tx, p, grid, stream)
-                        : launch_variant<KP, false, false, TWO, true>(tq, tx, p, grid, stream);
+            return is_l2 ? launch_op<KP, true, TWO, true>(op, tq, tx, p, grid, stream)
+                         : launch_op<KP, false, TWO, true>(op, tq, tx, p, grid, stream);
         }
     }
-    if (is_l2) {
-        return tf32 ? launch_variant<KP, true, true, TWO>(tq, tx, p, grid, stream)
-                    : launch_variant<KP, true, false, TWO>(tq, tx, p, grid, stream);
-    }
-    return tf32 ? launch_variant<KP, false, true, TWO>(tq, tx, p, grid, stream)
-                : launch_variant<KP, false, false, TWO>(tq, tx, p, grid, stream);
+    return is_l2 ? launch_op<KP, true, TWO>(op, tq, tx, p, grid, stream) : launch_op<KP, false, TWO>(op, tq, tx, p, grid, stream);
 }
 
 template <bool TWO>
-int launch_two(int kp, bool is_l2, bool tf32, const CUtensorMap& tq, const CUtensorMap& tx, const FilterParams& p, int grid,
+int launch_two(int kp, bool is_l2, Op op, const CUtensorMap& tq, const CUtensorMap& tx, const FilterParams& p, int grid,
                cudaStream_t stream) {
     switch (kp) {
-        case 16: return launch_kp<16, TWO>(is_l2, tf32, tq, tx, p, grid, stream);
-        case 32: return launch_kp<32, TWO>(is_l2, tf32, tq, tx, p, grid, stream);
-        case 64: return launch_kp<64, TWO>(is_l2, tf32, tq, tx, p, grid, stream);
-        case 72: return launch_kp<72, TWO>(is_l2, tf32, tq, tx, p, grid, stream);
+        case 16: return launch_kp<16, TWO>(is_l2, op, tq, tx, p, grid, stream);
+        case 32: return launch_kp<32, TWO>(is_l2, op, tq, tx, p, grid, stream);
+        case 64: return launch_kp<64, TWO>(is_l2, op, tq, tx, p, grid, stream);
+        case 72: return launch_kp<72, TWO>(is_l2, op, tq, tx, p, grid, stream);
         default: set_error("internal: unsupported candidate capacity %d", kp); return B2_EINVAL;
     }
 }
@@ -929,13 +950,13 @@ int launch_knn_filter(const MatView& X, const void* q_filt, int64_t q_pitch, int
         set_error("matrix too large for 32-bit row ids (n=%lld nq=%lld)", (long long)X.n, (long long)nq);
         return B2_ERANGE;
     }
-    const bool tf32 = X.filt_dtype == B2_F32;
-    const int kb_elems = KB_BYTES / (tf32 ? 4 : 2);
+    const Op op = filter_op(X.filt_dtype);
+    const int kb_elems = KB_BYTES / op_bytes(op);
     CUtensorMap tq, tx;
     const int64_t op_cols = X.d;
-    B2_TRY(make_tmap(&tq, q_filt, tf32, nq, op_cols, q_pitch, BLOCK_M));
+    B2_TRY(make_tmap(&tq, q_filt, op, nq, op_cols, q_pitch, BLOCK_M));
     // pair mode: each CTA of the pair loads HALF of the 256-row corpus tile (and multicasts it to both)
-    B2_TRY(make_tmap(&tx, X.filt, tf32, X.n, op_cols, X.filt_pitch, two_cta ? BLOCK_N / 2 : BLOCK_N));
+    B2_TRY(make_tmap(&tx, X.filt, op, X.n, op_cols, X.filt_pitch, two_cta ? BLOCK_N / 2 : BLOCK_N));
     FilterParams p;
     p.xnorm = X.norm2;
     p.cand_score = cand_score;
@@ -980,10 +1001,10 @@ int launch_knn_filter(const MatView& X, const void* q_filt, int64_t q_pitch, int
     int rc;
     if (two_cta) {
         const int pairs = (int)std::min<int64_t>(items, sm_count(device) / 2);
-        rc = launch_two<true>(kp, is_l2, tf32, tq, tx, p, 2 * pairs, stream);
+        rc = launch_two<true>(kp, is_l2, op, tq, tx, p, 2 * pairs, stream);
     } else {
         const int grid = (int)std::min<int64_t>(items, sm_count(device));
-        rc = launch_two<false>(kp, is_l2, tf32, tq, tx, p, grid, stream);
+        rc = launch_two<false>(kp, is_l2, op, tq, tx, p, grid, stream);
     }
     return rc;
 }
@@ -1005,11 +1026,11 @@ int launch_pair_filter(const MatView& X, float thr, int part, int nparts, int32_
         set_error("matrix too large for 32-bit row ids (n=%lld)", (long long)X.n);
         return B2_ERANGE;
     }
-    const bool tf32 = X.filt_dtype == B2_F32;
-    const int kb_elems = KB_BYTES / (tf32 ? 4 : 2);
+    const Op op = filter_op(X.filt_dtype);
+    const int kb_elems = KB_BYTES / op_bytes(op);
     CUtensorMap tq, tx;
-    B2_TRY(make_tmap(&tq, X.filt, tf32, X.n, X.d, X.filt_pitch, BLOCK_M));
-    B2_TRY(make_tmap(&tx, X.filt, tf32, X.n, X.d, X.filt_pitch, BLOCK_N));
+    B2_TRY(make_tmap(&tq, X.filt, op, X.n, X.d, X.filt_pitch, BLOCK_M));
+    B2_TRY(make_tmap(&tx, X.filt, op, X.n, X.d, X.filt_pitch, BLOCK_N));
     FilterParams p;
     memset(&p, 0, sizeof(p));
     p.nq = (int32_t)X.n;
@@ -1017,7 +1038,7 @@ int launch_pair_filter(const MatView& X, float thr, int part, int nparts, int32_
     p.num_kb = (int32_t)ceil_div(X.d, kb_elems);
     static const bool two = [] { const char* e = getenv("B2_PAIR_2CTA"); return e ? atoi(e) != 0 : true; }();  // default: CTA pairs
     const bool two_cta = two && ceil_div(X.n, BLOCK_M) >= 2;
-    if (two_cta) B2_TRY(make_tmap(&tx, X.filt, tf32, X.n, X.d, X.filt_pitch, BLOCK_N / 2));  // each CTA stages half a corpus tile
+    if (two_cta) B2_TRY(make_tmap(&tx, X.filt, op, X.n, X.d, X.filt_pitch, BLOCK_N / 2));  // each CTA stages half a corpus tile
     p.n_mtiles = (int32_t)ceil_div(X.n, BLOCK_M);
     p.n_munits = two_cta ? (p.n_mtiles + 1) / 2 : p.n_mtiles;
     p.n_ntiles = (int32_t)ceil_div(X.n, BLOCK_N);
@@ -1044,12 +1065,17 @@ int launch_pair_filter(const MatView& X, float thr, int part, int nparts, int32_
     p.pair_items = (int32_t)items;
     if (items <= 0) return B2_OK;
     const int grid = two_cta ? 2 * (int)std::min<int64_t>(items, sm_count(device) / 2) : (int)std::min<int64_t>(items, sm_count(device));
-    if (two_cta) {
-        return tf32 ? launch_cluster(pair_filter_kernel<true, true>, grid, PAIR_SMEM, true, tq, tx, p, stream)
-                    : launch_cluster(pair_filter_kernel<false, true>, grid, PAIR_SMEM, true, tq, tx, p, stream);
+    switch (op) {
+        case Op::TF32:
+            return two_cta ? launch_cluster(pair_filter_kernel<Op::TF32, true>, grid, PAIR_SMEM, true, tq, tx, p, stream)
+                           : launch_cluster(pair_filter_kernel<Op::TF32, false>, grid, PAIR_SMEM, false, tq, tx, p, stream);
+        case Op::BF16:
+            return two_cta ? launch_cluster(pair_filter_kernel<Op::BF16, true>, grid, PAIR_SMEM, true, tq, tx, p, stream)
+                           : launch_cluster(pair_filter_kernel<Op::BF16, false>, grid, PAIR_SMEM, false, tq, tx, p, stream);
+        default:  // Op::F16
+            return two_cta ? launch_cluster(pair_filter_kernel<Op::F16, true>, grid, PAIR_SMEM, true, tq, tx, p, stream)
+                           : launch_cluster(pair_filter_kernel<Op::F16, false>, grid, PAIR_SMEM, false, tq, tx, p, stream);
     }
-    return tf32 ? launch_cluster(pair_filter_kernel<true, false>, grid, PAIR_SMEM, false, tq, tx, p, stream)
-                : launch_cluster(pair_filter_kernel<false, false>, grid, PAIR_SMEM, false, tq, tx, p, stream);
 }
 
 }  // namespace b2

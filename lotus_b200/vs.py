@@ -77,24 +77,51 @@ class BF16Backed(np.ndarray):
         return np.ascontiguousarray(f32, dtype=np.float32).view(BF16Backed)
 
 
-def _to_host_matrix(a: Any, want_bf16: bool, exact_bf16_ok: bool = False, scratch: "dict | None" = None):
+def f32_to_f16_checked(f: np.ndarray) -> np.ndarray:
+    """float32 -> float16, round to nearest even. A finite value that would overflow to inf raises ValueError (|v| >= 65520):
+    an fp16 store must hold the user's numbers, not infinities."""
+    with np.errstate(over="ignore"):
+        h = f.astype(np.float16)
+    bad = np.isinf(h) & np.isfinite(f)
+    if bad.any():
+        v = f[bad].flat[0]
+        raise ValueError(f"value {v!r} is outside the float16 range (|v| < 65520); use dtype='f32' or 'bf16' for these embeddings")
+    return h
+
+
+def _to_host_matrix(a: Any, want_bf16: bool, exact_bf16_ok: bool = False, scratch: "dict | None" = None,
+                    want_f16: bool = False, pass_f16: bool = False):
     """-> (array for the C-ABI, native dtype code, float32 view of the stored values).
     exact_bf16_ok: when every float32 value is bfloat16-representable (e.g. vectors fetched from a bf16 index,
     sem_sim_join.py:112-118 -> :130-134) ship the exact 2-byte patterns instead: half the H2D bytes and the exact-operand
-    error bound in the certificate. Decided from the values themselves on every call (one threaded host pass)."""
+    error bound in the certificate. Decided from the values themselves on every call (one threaded host pass).
+    want_f16: store as float16 (float16 input as it is, anything else rounded once; overflow raises ValueError).
+    pass_f16: float16 input (numpy or torch) is shipped as it is, as 2-byte F16 operands (queries: exact in fp32)."""
     try:
         import torch
         if isinstance(a, torch.Tensor):
             t = a.detach()
-            if t.dtype == torch.bfloat16 or want_bf16:
+            if t.dtype == torch.float16 and (want_f16 or pass_f16) and not want_bf16:
+                a = t.contiguous().cpu().numpy()  # float16 ndarray: handled below
+            elif t.dtype == torch.bfloat16 or want_bf16:
                 bits = t.to(torch.bfloat16).contiguous().cpu().view(torch.int16).numpy().view(np.uint16)
                 return bits, nv.BF16, nv.bf16_bits_to_f32(bits)
-            a = t.to(torch.float32).contiguous().cpu().numpy()
+            else:
+                a = t.to(torch.float32).contiguous().cpu().numpy()
     except ImportError:  # pragma: no cover
         pass
-    f = np.ascontiguousarray(np.asarray(a), dtype=np.float32)  # faiss casts whatever it is given to float32
+    arr = np.asarray(a)
+    if arr.dtype == np.float16 and (want_f16 or pass_f16) and not want_bf16:
+        if arr.ndim != 2:
+            raise ValueError(f"embeddings must be 2-D, got shape {arr.shape}")
+        h = np.ascontiguousarray(arr)
+        return h, nv.F16, h.astype(np.float32)
+    f = np.ascontiguousarray(arr, dtype=np.float32)  # faiss casts whatever it is given to float32
     if f.ndim != 2:
         raise ValueError(f"embeddings must be 2-D, got shape {f.shape}")
+    if want_f16:
+        h = f32_to_f16_checked(f)
+        return h, nv.F16, h.astype(np.float32)
     if want_bf16:
         bits = nv.f32_to_bf16_bits(f)
         return bits, nv.BF16, nv.bf16_bits_to_f32(bits)
@@ -152,7 +179,7 @@ class MultiDeviceIndex:
         ids = np.asarray(ids, dtype=np.int64)
         if len(ids) and (ids.min() < 0 or ids.max() >= self.n):
             raise nv.NativeError(nv.ERANGE, f"ids contains a position outside [0, {self.n})")
-        out = np.empty((len(ids), self.d), dtype=np.float32 if self.dtype == nv.F32 else np.uint16)
+        out = np.empty((len(ids), self.d), dtype=nv.storage_dtype(self.dtype))
         for g, (lo, hi) in enumerate(self.bounds):
             m = (ids >= lo) & (ids < hi)
             if m.any():
@@ -196,7 +223,9 @@ class B200VS(VS):
 
     Args mirror FaissVS(factory_string="Flat", metric=faiss.METRIC_INNER_PRODUCT) (faiss_vs.py:14).
     dtype: "f32" (store what faiss would: float32), "bf16" (round the corpus to bfloat16 once; exact search
-    over those values), or "auto" (bf16 only when handed a bf16 tensor).
+    over those values), "f16" (store float16: float16 embeddings as they are, anything else rounded once, and a value
+    outside float16's range raises ValueError; searched at the bf16 rate with results equal to faiss on the float32
+    upcast of the stored values), or "auto" (bf16 only when handed a bf16 tensor, float32 otherwise).
     """
 
     accepts_id_arrays = True  # `ids=` may be a numpy int64 array (the operators then skip building a Python list)
@@ -208,8 +237,8 @@ class B200VS(VS):
             raise ValueError(f"B200VS implements the flat (exact) index only; factory_string={factory_string!r}")
         if metric not in (METRIC_INNER_PRODUCT, METRIC_L2):
             raise ValueError("metric must be METRIC_INNER_PRODUCT (0) or METRIC_L2 (1)")
-        if dtype not in ("auto", "f32", "bf16"):
-            raise ValueError("dtype must be 'auto', 'f32' or 'bf16'")
+        if dtype not in ("auto", "f32", "bf16", "f16"):
+            raise ValueError("dtype must be 'auto', 'f32', 'bf16' or 'f16'")
         self.factory_string = factory_string
         self.metric = metric
         self.dtype = dtype
@@ -231,16 +260,23 @@ class B200VS(VS):
             if t is not None:
                 import torch
                 want16 = want16 or (self.dtype == "auto" and t.dtype == torch.bfloat16)
-            host, code, _ = _to_host_matrix(embeddings, want16)
+            host, code, _ = _to_host_matrix(embeddings, want16, want_f16=self.dtype == "f16")
             return MultiDeviceIndex(host, code, self.metric, self.devices)  # type: ignore[return-value]
         if t is not None and t.dim() == 2 and t.device.index == self.device:
-            # device hand-off: the encoder's output never visits the host on its way into the index
+            # device hand-off: the encoder's output never visits the host on its way into the index (a tensor that
+            # already has the store's type is read in place)
             import torch
-            want = torch.bfloat16 if (self.dtype == "bf16" or (self.dtype == "auto" and t.dtype == torch.bfloat16)) else torch.float32
-            t = t.detach().to(want).contiguous()
-            return nv.Index(None, nv.BF16 if want == torch.bfloat16 else nv.F32, self.metric, self.device,
-                            on_device_ptr=t.data_ptr(), n=t.shape[0], d=t.shape[1])
-        host, code, _ = _to_host_matrix(embeddings, self.dtype == "bf16")
+            if self.dtype == "f16":
+                want = torch.float16
+            else:
+                want = torch.bfloat16 if (self.dtype == "bf16" or (self.dtype == "auto" and t.dtype == torch.bfloat16)) else torch.float32
+            src = t.detach()
+            t = src.to(want).contiguous()
+            if want == torch.float16 and src.dtype != torch.float16 and bool((torch.isinf(t) & torch.isfinite(src)).any()):
+                raise ValueError("embeddings hold values outside the float16 range (|v| < 65520); use dtype='f32' or 'bf16'")
+            code = {torch.float32: nv.F32, torch.bfloat16: nv.BF16, torch.float16: nv.F16}[want]
+            return nv.Index(None, code, self.metric, self.device, on_device_ptr=t.data_ptr(), n=t.shape[0], d=t.shape[1])
+        host, code, _ = _to_host_matrix(embeddings, self.dtype == "bf16", want_f16=self.dtype == "f16")
         return nv.Index(host, code, self.metric, self.device)
 
     def _remember(self, index_dir: str, idx: nv.Index, vecs: Any) -> None:
@@ -311,7 +347,9 @@ class B200VS(VS):
         idx = self._entry_for(index_dir)
         ids_a = np.asarray(list(ids) if not isinstance(ids, np.ndarray) else ids, dtype=np.int64)
         out = idx.gather(ids_a)
-        return BF16Backed.wrap(nv.bf16_bits_to_f32(out)) if idx.dtype == nv.BF16 else out
+        if idx.dtype == nv.BF16:
+            return BF16Backed.wrap(nv.bf16_bits_to_f32(out))
+        return out  # float32, or the float16 values of an fp16 index (like pickle.load(vecs)[ids] of float16 vecs)
 
     def __call__(self, query_vectors: Any, K: int, ids: list[int] | None = None, **kwargs: Any) -> RMOutput:
         """faiss_vs.py:43-77. Returns float32 distances [Q,K] and int64 indices [Q,K] (global ids; -1 = no result).
@@ -322,7 +360,8 @@ class B200VS(VS):
         t = _cuda_tensor(query_vectors)
         if t is not None and ids_a is None and t.dim() == 2 and t.device.index == self.device and not isinstance(self.b2_index, MultiDeviceIndex):
             return self._call_device(t, int(K))
-        q, code, _ = _to_host_matrix(query_vectors, False, exact_bf16_ok=self.b2_index.dtype == nv.BF16, scratch=self._scratch)
+        q, code, _ = _to_host_matrix(query_vectors, False, exact_bf16_ok=self.b2_index.dtype == nv.BF16, scratch=self._scratch,
+                                     pass_f16=True)
         if q.shape[1] != self.b2_index.d:
             raise ValueError(f"query dimension {q.shape[1]} does not match the index dimension {self.b2_index.d}")
         try:
@@ -340,8 +379,8 @@ class B200VS(VS):
         if t.shape[1] != self.b2_index.d:
             raise ValueError(f"query dimension {t.shape[1]} does not match the index dimension {self.b2_index.d}")
         q = t.detach()
-        q = q.contiguous() if q.dtype in (torch.float32, torch.bfloat16) else q.to(torch.float32).contiguous()
-        code = nv.BF16 if q.dtype == torch.bfloat16 else nv.F32
+        q = q.contiguous() if q.dtype in (torch.float32, torch.bfloat16, torch.float16) else q.to(torch.float32).contiguous()
+        code = {torch.float32: nv.F32, torch.bfloat16: nv.BF16, torch.float16: nv.F16}[q.dtype]
         out_s = torch.empty((q.shape[0], K), dtype=torch.float32, device=q.device)
         out_i = torch.empty((q.shape[0], K), dtype=torch.int64, device=q.device)
         try:
