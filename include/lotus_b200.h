@@ -196,12 +196,13 @@ B2_API int b2_host_bf16_to_f32(const uint16_t* x, int64_t count, float* out);
 
 /* The filter kernel's work schedule for a shape (no device work; used by the CPU tests): kp = candidate-list capacity (0 = the
  * shape goes to the dense path), n_splits = corpus splits, units_whole = leading query units that sweep the whole corpus as one
- * item each (two-phase schedule), two_cta = CTA-pair mode. */
+ * item each (two-phase schedule), two_cta = CTAs per cluster (1 = single CTAs; otherwise a query unit is two query tiles and
+ * there are num_sms / 2 workers, CTA pairs). */
 B2_API int b2_debug_filter_plan(int64_t nq, int64_t n, int32_t k, int32_t num_sms, int32_t* kp, int32_t* n_splits,
                          int32_t* units_whole, int32_t* two_cta);
 /* The filter kernel's raw candidate lists for host queries q[nq,d] (q_dtype), planned and launched exactly as a search does
  * (level 0; level 1 = the tf32 second level of an fp32 index, which drops its bf16 copy) or, with top1 != 0, as the k-means
- * assignment does (register top-2 epilogue). plan[8] receives: use_filter, kp, n_splits, units_whole, two_cta, two_level,
+ * assignment does (register top-2 epilogue). plan[8] receives: use_filter, kp, n_splits, units_whole, cluster, two_level,
  * filter operand dtype, query chunks; *rel_eps the filter's error bound relative to |q|*|x|. With every list buffer non-NULL
  * and use_filter set, the filter runs and fills (HOST buffers) cand_score / cand_id [nq, n_splits, 2 sets, kp/2] and
  * cand_thr [nq, n_splits, 2]; with any of them NULL only the plan is reported. B2_ERANGE when nq needs more than one query

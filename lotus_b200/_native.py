@@ -124,10 +124,12 @@ def require_device() -> None:
 
 
 def filter_plan(nq: int, n: int, k: int, num_sms: int = 132) -> dict:
-    """The filter kernel's schedule for a shape (host logic only, no device needed)."""
-    kp, ns, uw, two = ctypes.c_int32(), ctypes.c_int32(), ctypes.c_int32(), ctypes.c_int32()
-    check(lib().b2_debug_filter_plan(nq, n, k, num_sms, ctypes.byref(kp), ctypes.byref(ns), ctypes.byref(uw), ctypes.byref(two)))
-    return {"kp": kp.value, "n_splits": ns.value, "units_whole": uw.value, "two_cta": bool(two.value)}
+    """The filter kernel's schedule for a shape (host logic only, no device needed). two_cta: cluster mode, in which a query
+    unit is two query tiles and a worker a CTA pair (num_sms / 2 of them); cluster: CTAs per cluster (a cluster of four runs
+    two workers in lockstep)."""
+    kp, ns, uw, cl = ctypes.c_int32(), ctypes.c_int32(), ctypes.c_int32(), ctypes.c_int32()
+    check(lib().b2_debug_filter_plan(nq, n, k, num_sms, ctypes.byref(kp), ctypes.byref(ns), ctypes.byref(uw), ctypes.byref(cl)))
+    return {"kp": kp.value, "n_splits": ns.value, "units_whole": uw.value, "two_cta": cl.value > 1, "cluster": cl.value}
 
 
 def filter_eps(store_dtype: int, filt_dtype: int, q_dtype: int, d: int) -> tuple[float, float]:
@@ -289,7 +291,7 @@ class Index:
     def filter_lists(self, q: np.ndarray, k: int, q_dtype: int = F32, top1: bool = False, level: int = 0,
                      plan_only: bool = False) -> dict:
         """The filter kernel's raw candidate lists for host queries, run as a search (or, with top1, the k-means assignment)
-        runs it: the plan (use_filter, kp, n_splits, units_whole, two_cta, two_level, filt_dtype, rel_eps) plus, unless
+        runs it: the plan (use_filter, kp, n_splits, units_whole, two_cta, cluster, two_level, filt_dtype, rel_eps) plus, unless
         plan_only or the plan declines the filter, score/id [nq, n_splits, 2, kp/2] and thr [nq, n_splits, 2]."""
         q = np.ascontiguousarray(q)
         nq = q.shape[0]
@@ -299,7 +301,8 @@ class Index:
         eps = ctypes.c_float()
         L = lib()
         check(L.b2_debug_filter_lists(self._h, _ptr(q), nq, q_dtype, k, int(top1), level, plan, ctypes.byref(eps), None, None, None))
-        out = {"use_filter": bool(plan[0]), "kp": plan[1], "n_splits": plan[2], "units_whole": plan[3], "two_cta": bool(plan[4]),
+        out = {"use_filter": bool(plan[0]), "kp": plan[1], "n_splits": plan[2], "units_whole": plan[3], "two_cta": plan[4] > 1,
+               "cluster": plan[4],
                "two_level": bool(plan[5]), "filt_dtype": plan[6], "rel_eps": float(eps.value)}
         if plan_only or not out["use_filter"]:
             return out

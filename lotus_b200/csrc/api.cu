@@ -130,7 +130,8 @@ __global__ void fill_pad_kernel(float* sc, int64_t* id, int64_t total, float pad
 
 // The filter run of a search: for an fp32 store with a bf16 copy (X.filt16) and a small k it is the FIRST level of a two-level
 // search (bf16 filter, longer candidate list). Every caller filters exactly as planned here; b2_debug_filter_plan reports it.
-int plan_filter(const MatView& X_in, const void* q, int q_dtype, int64_t nq, int k, bool top1, int num_sms, FilterPlan& p) {
+int plan_filter(const MatView& X_in, const void* q, int q_dtype, int64_t nq, int k, bool top1, int device, FilterPlan& p,
+                int model_sms) {
     p = FilterPlan();
     p.q = q;
     p.q_dtype = q_dtype;
@@ -165,9 +166,11 @@ int plan_filter(const MatView& X_in, const void* q, int q_dtype, int64_t nq, int
         FilterChunk c;
         c.q0 = q0;
         c.nq = std::min<int64_t>(p.chunk, nq - q0);
-        c.two_cta = filter_use_pair(c.nq);
+        c.cluster = filter_cluster(c.nq, X.n, top1);
+        if (model_sms > 0) c.workers = std::max(1, model_sms / c.cluster) * (c.cluster > 2 ? c.cluster / 2 : 1);
+        else B2_TRY(filter_workers(device, p.kp, c.cluster, &c.workers));
         // the k-means top-2 epilogue keeps the uniform split schedule
-        c.n_splits = filter_choose_splits(c.nq, X.n, num_sms, c.two_cta, top1, p.min_splits, top1 ? nullptr : &c.units_whole);
+        c.n_splits = filter_choose_splits(c.nq, X.n, c.workers, c.cluster, top1, p.min_splits, top1 ? nullptr : &c.units_whole);
         if (c.n_splits <= 0) {
             set_error("internal: no valid corpus split for k=%d over %lld rows", k, (long long)X.n);
             return B2_EINVAL;
@@ -189,8 +192,9 @@ int run_filter(b2_index* idx, const FilterPlan& p, const FilterChunk& c, int met
     B2_TRY(idx->cand_id.ensure((size_t)c.nq * c.n_splits * p.kp * sizeof(int32_t)));
     B2_TRY(idx->cand_thr.ensure((size_t)c.nq * c.n_splits * 2 * sizeof(float)));  // two epilogue sets per split
     B2_CUDA(cudaEventRecord(idx->ev0, st));
-    B2_TRY(launch_knn_filter(X, q_filt, p.q_pitch, c.nq, metric, p.kp, c.n_splits, c.two_cta, idx->cand_score.as<float>(),
-                             idx->cand_id.as<int32_t>(), idx->cand_thr.as<float>(), idx->device, st, p.top1, c.units_whole));
+    B2_TRY(launch_knn_filter(X, q_filt, p.q_pitch, c.nq, metric, p.kp, c.n_splits, c.cluster, c.workers,
+                             idx->cand_score.as<float>(), idx->cand_id.as<int32_t>(), idx->cand_thr.as<float>(), st, p.top1,
+                             c.units_whole));
     B2_CUDA(cudaEventRecord(idx->ev1, st));
     return B2_OK;
 }
@@ -258,7 +262,7 @@ int search_core(b2_index* idx, const MatView& X_in, int metric, const void* q_de
         return B2_OK;
     }
     FilterPlan p;
-    B2_TRY(plan_filter(X_in, q_dev, q_dtype, nq, k, false, sm_count(idx->device), p));
+    B2_TRY(plan_filter(X_in, q_dev, q_dtype, nq, k, false, idx->device, p));
     const MatView& X = p.X;
     if (!p.use_filter) {
         if (k > dense_max_k()) {
@@ -561,7 +565,7 @@ int b2_index_search_stage1_dev(b2_index* idx, const void* q_dev, int64_t nq, int
     sg.active = true;
     const MatView& X = idx->view;
     FilterPlan& p = sg.plan;
-    B2_TRY(plan_filter(X, q_dev, q_dtype, nq, k, false, sm_count(idx->device), p));
+    B2_TRY(plan_filter(X, q_dev, q_dtype, nq, k, false, idx->device, p));
     if (!p.use_filter || p.two_level || p.chunks.size() != 1 || 2 * p.chunks[0].n_splits * (p.kp / 2) > shard_lower_bound_max_entries() ||
         j > k) {
         return launch_fill_f32(lower_dev, nq, -INFINITY, st);  // stage 2 will run the plain search
@@ -668,8 +672,9 @@ int b2_host_bf16_to_f32(const uint16_t* x, int64_t count, float* out) {
 }
 
 // The filter's work schedule for a (queries, rows, k) shape on `num_sms` SMs, as plan_filter decides it for a bf16 index (the
-// first query chunk when the batch takes several) — no device work: lets the CPU test-suite check that every (query unit,
-// corpus tile) pair is covered exactly once for the shapes the GPU tests do not reach.
+// first query chunk when the batch takes several) — no device work: the worker count is modelled as every SM in use, and
+// *two_cta receives the cluster size. Lets the CPU test-suite check that every (query unit, corpus tile) pair is covered
+// exactly once for the shapes the GPU tests do not reach.
 int b2_debug_filter_plan(int64_t nq, int64_t n, int32_t k, int32_t num_sms, int32_t* kp, int32_t* n_splits, int32_t* units_whole,
                          int32_t* two_cta) {
     if (nq <= 0 || n <= 0 || k <= 0 || num_sms <= 0 || !kp || !n_splits || !units_whole || !two_cta) { set_error("bad arguments"); return B2_EINVAL; }
@@ -678,12 +683,12 @@ int b2_debug_filter_plan(int64_t nq, int64_t n, int32_t k, int32_t num_sms, int3
     X.d = 8;
     X.dtype = X.filt_dtype = B2_BF16;
     FilterPlan p;
-    B2_TRY(plan_filter(X, nullptr, B2_BF16, nq, k, false, num_sms, p));
+    B2_TRY(plan_filter(X, nullptr, B2_BF16, nq, k, false, -1, p, num_sms));
     const FilterChunk c = p.use_filter ? p.chunks[0] : FilterChunk();
     *kp = p.use_filter ? p.kp : 0;
     *n_splits = c.n_splits;
     *units_whole = c.units_whole;
-    *two_cta = c.two_cta ? 1 : 0;
+    *two_cta = c.cluster;
     return B2_OK;
 }
 
@@ -704,13 +709,13 @@ int b2_debug_filter_lists(b2_index* idx, const void* q, int64_t nq, int32_t q_dt
         B2_CUDA(cudaMemcpyAsync(idx->q_in.p, q, qbytes, cudaMemcpyHostToDevice, st));
     }
     FilterPlan p;
-    B2_TRY(plan_filter(X, lists ? idx->q_in.p : nullptr, q_dtype, nq, k, top1 != 0, sm_count(idx->device), p));
+    B2_TRY(plan_filter(X, lists ? idx->q_in.p : nullptr, q_dtype, nq, k, top1 != 0, idx->device, p));
     const FilterChunk c = p.use_filter ? p.chunks[0] : FilterChunk();
     plan[0] = p.use_filter ? 1 : 0;
     plan[1] = p.use_filter ? p.kp : 0;
     plan[2] = c.n_splits;
     plan[3] = c.units_whole;
-    plan[4] = c.two_cta ? 1 : 0;
+    plan[4] = c.cluster;
     plan[5] = p.two_level ? 1 : 0;
     plan[6] = p.X.filt_dtype;
     plan[7] = (int32_t)p.chunks.size();

@@ -138,10 +138,11 @@ struct MatView {
 // knn_filter_sm90.cu
 int filter_kp_for_k(int k);  // candidate-list capacity used for a given k, 0 = k too large for the filter
 int launch_knn_filter(const MatView& X, const void* q_filt, int64_t q_pitch, int64_t nq, int metric, int kp,
-                      int n_splits, bool two_cta, float* cand_score, int32_t* cand_id, float* cand_thr, int device,
+                      int n_splits, int cluster, int workers, float* cand_score, int32_t* cand_id, float* cand_thr,
                       cudaStream_t stream, bool top1 = false, int units_whole = 0);
-bool filter_use_pair(int64_t nq);
-int filter_choose_splits(int64_t nq, int64_t n, int num_sms, bool two_cta, bool top1 = false, int min_splits = 1,
+int filter_cluster(int64_t nq, int64_t n, bool top1);  // CTAs per cluster of a filter launch: nq queries, n corpus rows
+int filter_workers(int device, int kp, int cl, int* workers);  // co-resident clusters of that launch on the current device
+int filter_choose_splits(int64_t nq, int64_t n, int workers, int cl, bool top1 = false, int min_splits = 1,
                          int* units_whole = nullptr);  // 0: impossible; *units_whole > 0: two-phase schedule (see the definition)
 int filter_min_splits_for_k(int k);
 int sm_count(int device);  // multiprocessor count of a device, cached

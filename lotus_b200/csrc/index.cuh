@@ -92,7 +92,8 @@ struct DeviceGuard {
 // sharded search, the k-means assignment and b2_debug_filter_plan.
 struct FilterChunk {  // the queries [q0, q0 + nq) of the call, filtered by one launch
     int64_t q0 = 0, nq = 0;
-    bool two_cta = false;
+    int cluster = 1;      // CTAs per cluster (filter_cluster)
+    int workers = 0;      // workers of the persistent launch, the co-resident ones: CTA pairs in cluster mode (filter_workers)
     int n_splits = 0;
     int units_whole = 0;  // > 0: two-phase schedule (see filter_choose_splits)
 };
@@ -159,7 +160,9 @@ int search_core(b2_index* idx, const MatView& X, int metric, const void* q_dev, 
                 const int64_t* id_map, int64_t id_offset, float* out_sc, int64_t* out_id, cudaStream_t st, int level = 0);
 float filter_rel_eps(int store_dtype, int filt_dtype, int q_dtype, int d);
 float filter_abs_eps(int store_dtype, int filt_dtype, int q_dtype, int d);
-int plan_filter(const MatView& X, const void* q, int q_dtype, int64_t nq, int k, bool top1, int num_sms, FilterPlan& plan);
+// model_sms > 0: plan without a device, modelling the workers as model_sms SMs all in use (b2_debug_filter_plan)
+int plan_filter(const MatView& X, const void* q, int q_dtype, int64_t nq, int k, bool top1, int device, FilterPlan& plan,
+                int model_sms = 0);
 // prep one chunk's queries (unless streamed in place), size the candidate workspace and run the filter between idx->ev0 and ev1
 int run_filter(b2_index* idx, const FilterPlan& plan, const FilterChunk& c, int metric, cudaStream_t st);
 // out[j] = x[ids[j]] for j < m, synchronised; ids outside [0, n) -> B2_ERANGE. scalar holds the device error flag.

@@ -671,7 +671,7 @@ int assign_points(b2_index* idx, const void* pts, const float* pnorm2, int64_t m
     B2_TRY(centroid_view(cent, k, d, idx->dtype, w, cv, st));
     const int dev_sms = sm_count(idx->device);
     FilterPlan p;
-    B2_TRY(plan_filter(cv, pts, idx->dtype, m, 1, /*top1=*/true, dev_sms, p));
+    B2_TRY(plan_filter(cv, pts, idx->dtype, m, 1, /*top1=*/true, idx->device, p));
     B2_TRY(w.flag_ids.ensure((size_t)std::min(m, p.chunk) * sizeof(int32_t)));
     B2_TRY(w.hard_ids.ensure((size_t)m * sizeof(int64_t)));
     B2_TRY(w.flag_count.ensure(64));

@@ -16,9 +16,12 @@
 //                    registers, 128 per thread) and runs the epilogue of those rows
 //   K-block = one 64-byte swizzle row (32 bf16 or fp16 / 16 tf32): wgmma k16 (bf16, fp16) or k8 (tf32), two per K-block.
 //   smem ring of NSTAGES x (A 8 KB + B 16 KB), mbarrier full/empty pairs.
-//   CTA pairs (default once there are two query tiles): a 2-CTA cluster takes two consecutive query tiles and sweeps the
-//   same corpus tiles; each CTA loads HALF of every corpus tile and TMA-multicasts it into both CTAs, so the corpus bytes
-//   read per SM drop by half. A stage is freed once the consumers of both CTAs are done with it.
+//   Clusters of CL CTAs (knn filter over a long corpus: FILTER_CL; k-means assignment, short corpora and dedup: CTA pairs; once
+//   a chunk has CL query tiles): the
+//   schedule's worker is a CTA pair that takes two consecutive query tiles (a query unit); a cluster of four runs two such
+//   workers in lockstep. Every CTA of a cluster sweeps the same corpus tiles, loads 1/CL of every corpus tile and
+//   TMA-multicasts it into all CL CTAs, so the corpus bytes each SM pulls from L2 drop CL-fold. A stage is freed once the
+//   consumers of every CTA of the cluster are done with it.
 //   Persistent: one CTA per SM, work item = (query unit, corpus split), query units fastest so that co-resident
 //   workers stream the same corpus tiles and hit them in L2.
 //
@@ -49,6 +52,12 @@ constexpr int MAX_STAGES = 8;
 constexpr int SMEM_LIMIT = 232448;  // 227 KB
 constexpr int SMEM_ALIGN_SLACK = 1024;  // the ring is aligned to 1024 B by hand
 constexpr int BAR_BYTES = 256;
+// CTAs per cluster of the knn filter: each CTA pulls A (8 KB) + B / FILTER_CL from L2 per K-block, 12 KB against 16 KB for a
+// pair, which lowers the energy per tile of a power-capped card. Clusters of 8 were no faster. Over a short corpus (the
+// k-means centroids: a few tiles per item) clusters of 4 were slower than pairs, so the k-means assignment (TOP1) and any
+// corpus of fewer than FILTER_CL_MIN_NTILES tiles keep CTA pairs (DESIGN §5).
+constexpr int FILTER_CL = 4;
+constexpr int FILTER_CL_MIN_NTILES = 32;
 constexpr int FILTER_MAX_K = 1000;  // largest k served by the filter (finalize keeps min(k + 32, 1024) survivors per query)
 
 // pending (not yet merged) candidates per (query row, set): a flush is triggered once any row holds PEND_FLUSH of them,
@@ -219,7 +228,8 @@ struct FilterParams {
     int32_t n;
     int32_t num_kb;        // K-blocks per tile = ceil(d / elements per 64 B)
     int32_t n_mtiles;      // ceil(nq / 128)
-    int32_t n_munits;      // schedulable query units: n_mtiles, or ceil(n_mtiles / 2) CTA pairs
+    int32_t n_munits;      // schedulable query units: n_mtiles, or ceil(n_mtiles / 2) pairs of query tiles in cluster mode
+                           // (clusters of four: rounded so that the units cut into splits are even, see launch_knn_filter)
     int32_t n_splits;
     int32_t top1;             // host-side switch only: the TOP1 kernel variant is launched (k-means assignment)
     int32_t tiles_per_split;  // corpus tiles (of 256 rows) per split
@@ -246,22 +256,29 @@ struct Ring {
     uint64_t *full_bar, *empty_bar;
 };
 
-// Persistent schedule. A "worker" is a CTA (or a CTA pair); item = (query unit, corpus split), unit fastest so that
-// co-resident workers stream the same corpus tiles and share them in L2.
+// Persistent schedule. A "worker" is a CTA pair in cluster mode (a single CTA when CL == 1); item = (query unit, corpus
+// split), unit fastest so that co-resident workers stream the same corpus tiles and share them in L2. A cluster of four holds
+// workers 2c and 2c + 1, which must sweep the same corpus tiles item for item: they do when the number of items is even and
+// the units cut into splits are even in number (the host rounds them up), since their items 2c + k W and 2c + 1 + k W are
+// then the same split of neighbouring units (W, the worker count, is even).
 struct Sched {
-    int worker, n_workers, rank;  // rank = CTA rank inside the pair (0 in single-CTA mode)
+    int worker, n_workers;
+    int rank;  // query tile of the unit this CTA takes (0 or 1; 0 in single-CTA mode)
+    int cta;   // CTA rank inside the cluster: which 1/CL of each corpus tile it loads
 };
-template <bool TWO>
+template <int CL>
 __device__ __forceinline__ Sched make_sched() {
     Sched sc;
-    if constexpr (TWO) {
+    if constexpr (CL > 1) {
         sc.worker = blockIdx.x >> 1;
         sc.n_workers = gridDim.x >> 1;
-        sc.rank = (int)cluster_ctarank();
+        sc.cta = (int)cluster_ctarank();
+        sc.rank = CL == 2 ? sc.cta : (sc.cta & 1);
     } else {
         sc.worker = blockIdx.x;
         sc.n_workers = gridDim.x;
         sc.rank = 0;
+        sc.cta = 0;
     }
     return sc;
 }
@@ -269,7 +286,7 @@ __device__ __forceinline__ int num_items(const FilterParams& p) {
     if (p.pair_mode) return p.pair_items;
     return p.units_whole + (p.n_munits - p.units_whole) * p.n_splits;
 }
-template <bool TWO>
+template <int CL>
 __device__ __forceinline__ void item_range(const FilterParams& p, const Sched& sc, int item, int& m_tile, int& split, int& t0,
                                            int& t1) {
     if (p.pair_mode) {
@@ -278,9 +295,9 @@ __device__ __forceinline__ void item_range(const FilterParams& p, const Sched& s
         const int grp = item / p.pair_group;
         const int first = (grp * p.nparts + p.part) * p.pair_group;
         const int unit = first + (item - grp * p.pair_group);
-        m_tile = TWO ? 2 * unit + sc.rank : unit;
+        m_tile = CL > 1 ? 2 * unit + sc.rank : unit;
         split = 0;
-        const int lead_tile = (p.pair_align ? first : unit) * (TWO ? 2 : 1);
+        const int lead_tile = (p.pair_align ? first : unit) * (CL > 1 ? 2 : 1);
         t0 = (lead_tile * BLOCK_M) / BLOCK_N;  // first corpus tile that can contain a column > row
         t1 = p.n_ntiles;
     } else {
@@ -297,13 +314,15 @@ __device__ __forceinline__ void item_range(const FilterParams& p, const Sched& s
             t0 = split * p.tiles_per_split;
             t1 = min(t0 + p.tiles_per_split, p.n_ntiles);
         }
-        m_tile = TWO ? 2 * unit + sc.rank : unit;
+        m_tile = CL > 1 ? 2 * unit + sc.rank : unit;  // past n_mtiles in a surplus unit: loads zeros, writes nothing
     }
 }
 
-// TMA producer: one lane (per CTA) streams (query tile, corpus tile) K-blocks into the smem ring. In a CTA pair each CTA
-// loads its own query rows and half of the corpus tile, multicast to both CTAs; every CTA's full barrier counts a whole stage.
-template <Op OP, int NSTAGES, bool TWO>
+// TMA producer: one lane (per CTA) streams (query tile, corpus tile) K-blocks into the smem ring. In a cluster each CTA
+// loads its own query rows and 1/CL of the corpus tile, multicast to every CTA; every CTA's full barrier counts a whole stage.
+// A piece of BLOCK_N / CL rows is a whole number of 512-byte SWIZZLE_64B periods, so the pieces tile the B stage exactly as
+// one full-tile box would.
+template <Op OP, int NSTAGES, int CL>
 __device__ __forceinline__ void producer_loop(const CUtensorMap* tmap_q, const CUtensorMap* tmap_x, const FilterParams& p,
                                               const Ring& r, const Sched& sc) {
     constexpr int KB_ELEMS = KB_BYTES / op_bytes(OP);
@@ -312,7 +331,7 @@ __device__ __forceinline__ void producer_loop(const CUtensorMap* tmap_q, const C
     uint32_t phase = 0;
     for (int item = sc.worker; item < n_items; item += sc.n_workers) {
         int m_tile, split, t0, t1;
-        item_range<TWO>(p, sc, item, m_tile, split, t0, t1);
+        item_range<CL>(p, sc, item, m_tile, split, t0, t1);
         for (int t = t0; t < t1; ++t) {
             for (int kb = 0; kb < p.num_kb; ++kb) {
                 mbar_wait(&r.empty_bar[stage], phase ^ 1);
@@ -320,9 +339,9 @@ __device__ __forceinline__ void producer_loop(const CUtensorMap* tmap_q, const C
                 uint8_t* sb = sa + STAGE_A_BYTES;
                 mbar_arrive_expect_tx(&r.full_bar[stage], STAGE_BYTES);
                 tma_load_2d(sa, tmap_q, &r.full_bar[stage], kb * KB_ELEMS, m_tile * BLOCK_M);
-                if constexpr (TWO)
-                    tma_load_2d_multicast(sb + sc.rank * (STAGE_B_BYTES / 2), tmap_x, &r.full_bar[stage], kb * KB_ELEMS,
-                                          t * BLOCK_N + sc.rank * (BLOCK_N / 2), (uint16_t)3);
+                if constexpr (CL > 1)
+                    tma_load_2d_multicast(sb + sc.cta * (STAGE_B_BYTES / CL), tmap_x, &r.full_bar[stage], kb * KB_ELEMS,
+                                          t * BLOCK_N + sc.cta * (BLOCK_N / CL), (uint16_t)((1u << CL) - 1));
                 else
                     tma_load_2d(sb, tmap_x, &r.full_bar[stage], kb * KB_ELEMS, t * BLOCK_N);
                 if (++stage == NSTAGES) {
@@ -334,20 +353,27 @@ __device__ __forceinline__ void producer_loop(const CUtensorMap* tmap_q, const C
     }
 }
 
-// a consumer warp is done reading stage s: one arrival per warp, in both CTAs of a pair (the peer multicasts into this stage)
-template <bool TWO>
-__device__ __forceinline__ void release_stage(const Ring& r, int s, int rank) {
+// a consumer warp is done reading stage s: one arrival per warp, in every CTA of the cluster (each of them multicasts into
+// this stage). A pair keeps lane 0 arriving locally and at the peer; larger clusters spread the arrivals over lanes 0..CL-1,
+// one remote arrive each, so a warp still issues one arrive instruction.
+template <int CL>
+__device__ __forceinline__ void release_stage(const Ring& r, int s, int cta) {
     __syncwarp();
-    if ((threadIdx.x & 31) == 0) {
-        mbar_arrive(&r.empty_bar[s]);
-        if constexpr (TWO) mbar_arrive_cluster(&r.empty_bar[s], (uint32_t)(rank ^ 1));
+    if constexpr (CL <= 2) {
+        if ((threadIdx.x & 31) == 0) {
+            mbar_arrive(&r.empty_bar[s]);
+            if constexpr (CL == 2) mbar_arrive_cluster(&r.empty_bar[s], (uint32_t)(cta ^ 1));
+        }
+    } else {
+        const uint32_t lane = threadIdx.x & 31;
+        if (lane < CL) mbar_arrive_cluster(&r.empty_bar[s], lane);
     }
 }
 
 // Consumer warpgroup g: acc = (query rows 64g..64g+63 of the stage's A tile) . (the 256 corpus rows)^T over all K-blocks of
 // one corpus tile. One wgmma group per K-block; a stage is released as soon as the group that read it has retired.
-template <Op OP, int NSTAGES, bool TWO>
-__device__ __forceinline__ void mma_tile(float (&acc)[128], const Ring& r, int num_kb, int g, int rank, int& stage, uint32_t& phase) {
+template <Op OP, int NSTAGES, int CL>
+__device__ __forceinline__ void mma_tile(float (&acc)[128], const Ring& r, int num_kb, int g, int cta, int& stage, uint32_t& phase) {
     const uint32_t a_off = (uint32_t)(g * WG_M * KB_BYTES);
     int prev = -1;
     for (int kb = 0; kb < num_kb; ++kb) {
@@ -362,7 +388,7 @@ __device__ __forceinline__ void mma_tile(float (&acc)[128], const Ring& r, int n
         wgmma_commit();
         if (prev >= 0) {
             wgmma_wait<1>();
-            release_stage<TWO>(r, prev, rank);
+            release_stage<CL>(r, prev, cta);
         }
         prev = stage;
         if (++stage == NSTAGES) {
@@ -372,11 +398,11 @@ __device__ __forceinline__ void mma_tile(float (&acc)[128], const Ring& r, int n
     }
     wgmma_wait<0>();
     acc_fence(acc);
-    release_stage<TWO>(r, prev, rank);
+    release_stage<CL>(r, prev, cta);
 }
 
 // barrier init shared by both kernels; returns after the block-wide (cluster-wide) sync
-template <int NSTAGES, bool TWO>
+template <int NSTAGES, int CL>
 __device__ __forceinline__ Ring setup_ring(uint8_t* smem, const CUtensorMap* tmap_q, const CUtensorMap* tmap_x) {
     Ring r;
     r.stage_base = smem;
@@ -387,20 +413,20 @@ __device__ __forceinline__ Ring setup_ring(uint8_t* smem, const CUtensorMap* tma
         tma_prefetch_desc(tmap_q);
         tma_prefetch_desc(tmap_x);
         for (int s = 0; s < NSTAGES; ++s) {
-            mbar_init(&r.full_bar[s], 1);  // the producer arms it; TMA (of both CTAs in a pair) completes the bytes
-            mbar_init(&r.empty_bar[s], TWO ? 2 * CONSUMER_WARPS : CONSUMER_WARPS);  // one arrival per consumer warp (of both CTAs)
+            mbar_init(&r.full_bar[s], 1);  // the producer arms it; TMA (of every CTA in a cluster) completes the bytes
+            mbar_init(&r.empty_bar[s], CL * CONSUMER_WARPS);  // one arrival per consumer warp of every CTA
         }
         fence_barrier_init();
     }
-    if constexpr (TWO) cluster_sync_all();  // the peer must see initialised barriers before any remote arrive / multicast
+    if constexpr (CL > 1) cluster_sync_all();  // the peers must see initialised barriers before any remote arrive / multicast
     else __syncthreads();
     return r;
 }
 
-template <bool TWO>
+template <int CL>
 __device__ __forceinline__ void teardown_ring() {
     __syncwarp();
-    if constexpr (TWO) cluster_sync_all();  // nobody leaves while the peer may still multicast into its smem or arrive on it
+    if constexpr (CL > 1) cluster_sync_all();  // nobody leaves while a peer may still multicast into its smem or arrive on it
 }
 
 __device__ __forceinline__ uint8_t* align_smem(uint8_t* raw) {
@@ -522,7 +548,7 @@ __device__ __forceinline__ void process8_top2(const float (&v)[8], int idx0, flo
     }
 }
 
-template <int KP, bool IS_L2, Op OP, bool TWO, bool TOP1 = false>
+template <int KP, bool IS_L2, Op OP, int CL, bool TOP1 = false>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 knn_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_x,
                   const FilterParams p) {
@@ -541,13 +567,13 @@ knn_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
     int32_t* pend_id_base = reinterpret_cast<int32_t*>(pend_sc_base + 2 * PEND_SET_STRIDE);
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-    const Ring ring = setup_ring<NSTAGES, TWO>(smem, &tmap_q, &tmap_x);
+    const Ring ring = setup_ring<NSTAGES, CL>(smem, &tmap_q, &tmap_x);
     const int n_items = num_items(p);
-    const Sched sc = make_sched<TWO>();
+    const Sched sc = make_sched<CL>();
 
     if (warp < 4) {
         setmaxnreg_dec<40>();
-        if (threadIdx.x == 0) producer_loop<OP, NSTAGES, TWO>(&tmap_q, &tmap_x, p, ring, sc);
+        if (threadIdx.x == 0) producer_loop<OP, NSTAGES, CL>(&tmap_q, &tmap_x, p, ring, sc);
     } else {
         setmaxnreg_inc<232>();
         // ===================== consumer warpgroup g: wgmma of 64 query rows, streaming top-KPH per (row, set) ==========
@@ -567,7 +593,7 @@ knn_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
         float acc[128];
         for (int item = sc.worker; item < n_items; item += sc.n_workers) {
             int m_tile, split, t0, t1;
-            item_range<TWO>(p, sc, item, m_tile, split, t0, t1);
+            item_range<CL>(p, sc, item, m_tile, split, t0, t1);
             if constexpr (!TOP1) {
 #pragma unroll 4
                 for (int i = 0; i < KPH; ++i) {
@@ -584,7 +610,7 @@ knn_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
             // lane fr + 8h + 16s
             float gthr[2][2] = {{-INFINITY, -INFINITY}, {-INFINITY, -INFINITY}};
             for (int t = t0; t < t1; ++t) {
-                mma_tile<OP, NSTAGES, TWO>(acc, ring, p.num_kb, g, sc.rank, stage, phase);
+                mma_tile<OP, NSTAGES, CL>(acc, ring, p.num_kb, g, sc.cta, stage, phase);
                 const int col0 = t * BLOCK_N;
                 const int ncols = min(BLOCK_N, p.n - col0);
 #pragma unroll
@@ -672,26 +698,26 @@ knn_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
         }
     }
 
-    teardown_ring<TWO>();
+    teardown_ring<CL>();
 }
 
 // ---- all-pairs threshold filter (sem_dedup): same mainloop, the epilogue emits (i, j) candidates -------------------
 constexpr int PAIR_STAGES = MAX_STAGES;
 constexpr int PAIR_SMEM = PAIR_STAGES * STAGE_BYTES + BAR_BYTES + SMEM_ALIGN_SLACK;
 
-template <Op OP, bool TWO>
+template <Op OP, int CL>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 pair_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_x, const FilterParams p) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = align_smem(smem_raw);
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-    const Ring ring = setup_ring<PAIR_STAGES, TWO>(smem, &tmap_q, &tmap_x);
+    const Ring ring = setup_ring<PAIR_STAGES, CL>(smem, &tmap_q, &tmap_x);
     const int n_items = num_items(p);
-    const Sched sc = make_sched<TWO>();
+    const Sched sc = make_sched<CL>();
     if (warp < 4) {
         setmaxnreg_dec<40>();
-        if (threadIdx.x == 0) producer_loop<OP, PAIR_STAGES, TWO>(&tmap_q, &tmap_x, p, ring, sc);
+        if (threadIdx.x == 0) producer_loop<OP, PAIR_STAGES, CL>(&tmap_q, &tmap_x, p, ring, sc);
     } else {
         setmaxnreg_inc<232>();
         const int g = (warp >> 2) - 1;
@@ -702,10 +728,10 @@ pair_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_cons
         float acc[128];
         for (int item = sc.worker; item < n_items; item += sc.n_workers) {
             int m_tile, split, t0, t1;
-            item_range<TWO>(p, sc, item, m_tile, split, t0, t1);
+            item_range<CL>(p, sc, item, m_tile, split, t0, t1);
             const int gi0 = m_tile * BLOCK_M + g * WG_M + wq * 16 + (lane >> 2);  // global rows gi0 and gi0 + 8 of this lane
             for (int t = t0; t < t1; ++t) {
-                mma_tile<OP, PAIR_STAGES, TWO>(acc, ring, p.num_kb, g, sc.rank, stage, phase);
+                mma_tile<OP, PAIR_STAGES, CL>(acc, ring, p.num_kb, g, sc.cta, stage, phase);
                 const int col0 = t * BLOCK_N + 2 * (lane & 3);
                 float mx = acc[0];
 #pragma unroll
@@ -727,7 +753,7 @@ pair_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_cons
             }
         }
     }
-    teardown_ring<TWO>();
+    teardown_ring<CL>();
 }
 
 // ---- host side ---------------------------------------------------------------------------------------------
@@ -790,7 +816,7 @@ int make_tmap(CUtensorMap* map, const void* base, Op op, int64_t rows, int64_t c
 }
 
 template <typename Kern>
-int launch_cluster(Kern kern, int grid, int smem, bool two, const CUtensorMap& tq, const CUtensorMap& tx, const FilterParams& p,
+int launch_cluster(Kern kern, int grid, int smem, int cl, const CUtensorMap& tq, const CUtensorMap& tx, const FilterParams& p,
                    cudaStream_t stream) {
     // the attribute is per DEVICE (not per process): set it on every launch — a microsecond — so that a process driving
     // several GPUs (B200VS(device=i) for several i) launches correctly on each of them
@@ -802,7 +828,7 @@ int launch_cluster(Kern kern, int grid, int smem, bool two, const CUtensorMap& t
     cfg.stream = stream;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = two ? 2 : 1;
+    attr[0].val.clusterDim.x = (unsigned)cl;
     attr[0].val.clusterDim.y = 1;
     attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr;
@@ -813,41 +839,79 @@ int launch_cluster(Kern kern, int grid, int smem, bool two, const CUtensorMap& t
     return B2_OK;
 }
 
-template <int KP, bool IS_L2, Op OP, bool TWO, bool TOP1 = false>
+template <int KP, bool IS_L2, Op OP, int CL, bool TOP1 = false>
 int launch_variant(const CUtensorMap& tq, const CUtensorMap& tx, const FilterParams& p, int grid, cudaStream_t stream) {
-    return launch_cluster(knn_filter_kernel<KP, IS_L2, OP, TWO, TOP1>, grid, smem_bytes(KP), TWO, tq, tx, p, stream);
+    return launch_cluster(knn_filter_kernel<KP, IS_L2, OP, CL, TOP1>, grid, smem_bytes(KP), CL, tq, tx, p, stream);
 }
 
-template <int KP, bool IS_L2, bool TWO, bool TOP1 = false>
+template <int KP, bool IS_L2, int CL, bool TOP1 = false>
 int launch_op(Op op, const CUtensorMap& tq, const CUtensorMap& tx, const FilterParams& p, int grid, cudaStream_t stream) {
     switch (op) {
-        case Op::TF32: return launch_variant<KP, IS_L2, Op::TF32, TWO, TOP1>(tq, tx, p, grid, stream);
-        case Op::BF16: return launch_variant<KP, IS_L2, Op::BF16, TWO, TOP1>(tq, tx, p, grid, stream);
-        default: return launch_variant<KP, IS_L2, Op::F16, TWO, TOP1>(tq, tx, p, grid, stream);  // Op::F16
+        case Op::TF32: return launch_variant<KP, IS_L2, Op::TF32, CL, TOP1>(tq, tx, p, grid, stream);
+        case Op::BF16: return launch_variant<KP, IS_L2, Op::BF16, CL, TOP1>(tq, tx, p, grid, stream);
+        default: return launch_variant<KP, IS_L2, Op::F16, CL, TOP1>(tq, tx, p, grid, stream);  // Op::F16
     }
 }
 
-template <int KP, bool TWO>
+template <int KP, int CL>
 int launch_kp(bool is_l2, Op op, const CUtensorMap& tq, const CUtensorMap& tx, const FilterParams& p, int grid,
               cudaStream_t stream) {
-    if constexpr (KP == 16) {
-        if (p.top1) {  // k == 1: register-resident top-2 epilogue
-            return is_l2 ? launch_op<KP, true, TWO, true>(op, tq, tx, p, grid, stream)
-                         : launch_op<KP, false, TWO, true>(op, tq, tx, p, grid, stream);
-        }
-    }
-    return is_l2 ? launch_op<KP, true, TWO>(op, tq, tx, p, grid, stream) : launch_op<KP, false, TWO>(op, tq, tx, p, grid, stream);
+    return is_l2 ? launch_op<KP, true, CL>(op, tq, tx, p, grid, stream) : launch_op<KP, false, CL>(op, tq, tx, p, grid, stream);
 }
 
-template <bool TWO>
-int launch_two(int kp, bool is_l2, Op op, const CUtensorMap& tq, const CUtensorMap& tx, const FilterParams& p, int grid,
-               cudaStream_t stream) {
+// k == 1 (k-means assignment, KP = 16): register-resident top-2 epilogue
+template <int CL>
+int launch_top1(bool is_l2, Op op, const CUtensorMap& tq, const CUtensorMap& tx, const FilterParams& p, int grid,
+                cudaStream_t stream) {
+    return is_l2 ? launch_op<16, true, CL, true>(op, tq, tx, p, grid, stream)
+                 : launch_op<16, false, CL, true>(op, tq, tx, p, grid, stream);
+}
+
+template <int CL>
+int launch_cl(int kp, bool is_l2, Op op, const CUtensorMap& tq, const CUtensorMap& tx, const FilterParams& p, int grid,
+              cudaStream_t stream) {
     switch (kp) {
-        case 16: return launch_kp<16, TWO>(is_l2, op, tq, tx, p, grid, stream);
-        case 32: return launch_kp<32, TWO>(is_l2, op, tq, tx, p, grid, stream);
-        case 64: return launch_kp<64, TWO>(is_l2, op, tq, tx, p, grid, stream);
-        case 72: return launch_kp<72, TWO>(is_l2, op, tq, tx, p, grid, stream);
+        case 16: return launch_kp<16, CL>(is_l2, op, tq, tx, p, grid, stream);
+        case 32: return launch_kp<32, CL>(is_l2, op, tq, tx, p, grid, stream);
+        case 64: return launch_kp<64, CL>(is_l2, op, tq, tx, p, grid, stream);
+        case 72: return launch_kp<72, CL>(is_l2, op, tq, tx, p, grid, stream);
         default: set_error("internal: unsupported candidate capacity %d", kp); return B2_EINVAL;
+    }
+}
+
+// Clusters of `cl` CTAs of `kern` that the current device holds at once. A GPC only holds whole clusters, and H100 GPCs do
+// not all hold a multiple of four SMs, so this can be less than sm_count / cl; a persistent grid sized past it would run a
+// trailing wave.
+template <typename Kern>
+int co_resident_clusters(Kern kern, int smem, int cl, int* n) {
+    B2_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3((unsigned)cl);
+    cfg.blockDim = dim3(NUM_THREADS);
+    cfg.dynamicSmemBytes = smem;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = (unsigned)cl;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    *n = 0;
+    B2_CUDA(cudaOccupancyMaxActiveClusters(n, kern, &cfg));
+    if (*n <= 0) {
+        set_error("the filter kernel fits no cluster of %d CTAs (%d B of shared memory each)", cl, smem);
+        return B2_ECUDA;
+    }
+    return B2_OK;
+}
+
+// every instantiation of one KP has the same block, shared memory and register budget, so the IP / bf16 one stands for all
+template <int KP>
+int co_resident_filter_clusters(int cl, int* n) {
+    switch (cl) {
+        case 1: return co_resident_clusters(knn_filter_kernel<KP, false, Op::BF16, 1>, smem_bytes(KP), cl, n);
+        case 2: return co_resident_clusters(knn_filter_kernel<KP, false, Op::BF16, 2>, smem_bytes(KP), cl, n);
+        default: return co_resident_clusters(knn_filter_kernel<KP, false, Op::BF16, FILTER_CL>, smem_bytes(KP), cl, n);
     }
 }
 
@@ -876,23 +940,49 @@ int filter_kp_for_k(int k) {
 // by the certificate (its discard bound reaches the k-th exact score) and that query takes the dense path.
 int filter_min_splits_for_k(int k) { return k <= 40 ? 1 : (int)ceil_div(k, 36); }
 
-// CTA pairs need at least two query tiles; B2_FILTER_2CTA=0/1 overrides the default.
-bool filter_use_pair(int64_t nq) {
+// Clusters of FILTER_CL CTAs over a long corpus, CTA pairs for the k-means assignment and short corpora; a cluster needs at
+// least that many query tiles. Smaller chunks, or B2_FILTER_2CTA=0, run single CTAs.
+int filter_cluster(int64_t nq, int64_t n, bool top1) {
     static int mode = -1;
     if (mode < 0) {
         const char* e = getenv("B2_FILTER_2CTA");
-        mode = e ? (atoi(e) != 0 ? 1 : 0) : 1;  // default: CTA pairs
+        mode = e ? (atoi(e) != 0 ? 1 : 0) : 1;  // default: clusters
     }
-    return mode == 1 && ceil_div(nq, BLOCK_M) >= 2;
+    const int cl = top1 || ceil_div(n, BLOCK_N) < FILTER_CL_MIN_NTILES ? 2 : FILTER_CL;
+    return mode == 1 && ceil_div(nq, BLOCK_M) >= cl ? cl : 1;
 }
 
-// Number of corpus splits: enough work items to fill the machine, and few idle workers in the last wave.
-// In pair mode a worker is a CTA pair and a query unit is two query tiles.
-int filter_choose_splits(int64_t nq, int64_t n, int num_sms, bool two_cta, bool top1, int min_splits, int* units_whole) {
+// Workers of one persistent filter launch with candidate capacity kp on the current device, which is `device`: as many as
+// are co-resident (CTA pairs in cluster mode, two per cluster of four; single CTAs otherwise), cached per device.
+int filter_workers(int device, int kp, int cl, int* workers) {
+    static int cached[64][3][4] = {};
+    const int ki = kp == 16 ? 0 : kp == 32 ? 1 : kp == 64 ? 2 : 3;
+    const int ci = cl == 1 ? 0 : cl == 2 ? 1 : 2;
+    int* slot = (device >= 0 && device < 64) ? &cached[device][ci][ki] : nullptr;
+    if (slot && *slot) {
+        *workers = *slot;
+        return B2_OK;
+    }
+    switch (kp) {
+        case 16: B2_TRY(co_resident_filter_clusters<16>(cl, workers)); break;
+        case 32: B2_TRY(co_resident_filter_clusters<32>(cl, workers)); break;
+        case 64: B2_TRY(co_resident_filter_clusters<64>(cl, workers)); break;
+        case 72: B2_TRY(co_resident_filter_clusters<72>(cl, workers)); break;
+        default: set_error("internal: unsupported candidate capacity %d", kp); return B2_EINVAL;
+    }
+    if (cl > 2) *workers *= cl / 2;
+    if (slot) *slot = *workers;
+    return B2_OK;
+}
+
+// Number of corpus splits: enough work items to fill the `workers` workers, and few idle workers in the last wave.
+// In cluster mode (cl > 1) a worker is a CTA pair and a query unit is two query tiles; in clusters of four the units cut into
+// splits are rounded up to an even number (see make_sched).
+int filter_choose_splits(int64_t nq, int64_t n, int workers, int cl, bool top1, int min_splits, int* units_whole) {
     if (units_whole) *units_whole = 0;
     const int64_t n_mtiles = ceil_div(nq, BLOCK_M);
-    const int64_t n_units = two_cta ? ceil_div(n_mtiles, 2) : n_mtiles;
-    const int64_t workers = two_cta ? std::max(1, num_sms / 2) : num_sms;
+    const int64_t n_units = cl > 1 ? ceil_div(n_mtiles, 2) : n_mtiles;
+    auto split_units = [cl](int64_t u) { return cl > 2 ? u + (u & 1) : u; };
     const int64_t n_ntiles = ceil_div(n, BLOCK_N);
     // cost model: an item costs its corpus tiles plus ~13 tile-times of list warm-up, the
     // kernel takes `waves` such items back to back, and every extra split adds two candidate lists per query to finalize
@@ -902,7 +992,7 @@ int filter_choose_splits(int64_t nq, int64_t n, int num_sms, bool two_cta, bool 
     for (int s = std::max(1, min_splits); s <= 256 && s <= n_ntiles; ++s) {
         const int64_t tps = ceil_div(n_ntiles, s);
         if (ceil_div(n_ntiles, tps) != s) continue;  // every split must receive tiles
-        const int64_t items = n_units * s;
+        const int64_t items = split_units(n_units) * s;
         const int64_t waves = ceil_div(items, workers);
         const double cost = (double)waves * ((double)tps + kWarmupTiles) * (1.0 + 0.004 * s);
         if (cost < best_cost - 1e-9) {
@@ -926,7 +1016,7 @@ int filter_choose_splits(int64_t nq, int64_t n, int num_sms, bool two_cta, bool 
             for (int s = 1; s <= 256 && s <= n_ntiles; ++s) {
                 const int64_t tps = ceil_div(n_ntiles, s);
                 if (ceil_div(n_ntiles, tps) != s) continue;
-                const int64_t waves_b = ceil_div(rem * s, workers);
+                const int64_t waves_b = ceil_div(split_units(rem) * s, workers);
                 const double cost = (cost_a + (double)waves_b * ((double)tps + kWarmupTiles)) * (1.0 + 0.002 * s);
                 if (cost < best2 - 1e-9) {
                     best2 = cost;
@@ -943,7 +1033,7 @@ int filter_choose_splits(int64_t nq, int64_t n, int num_sms, bool two_cta, bool 
 }
 
 int launch_knn_filter(const MatView& X, const void* q_filt, int64_t q_pitch, int64_t nq, int metric, int kp,
-                      int n_splits, bool two_cta, float* cand_score, int32_t* cand_id, float* cand_thr, int device,
+                      int n_splits, int cluster, int workers, float* cand_score, int32_t* cand_id, float* cand_thr,
                       cudaStream_t stream, bool top1, int units_whole) {
     if (nq <= 0 || X.n <= 0) return B2_OK;
     if (X.n > 0x7fffff00LL || nq > 0x7fffff00LL) {
@@ -955,8 +1045,8 @@ int launch_knn_filter(const MatView& X, const void* q_filt, int64_t q_pitch, int
     CUtensorMap tq, tx;
     const int64_t op_cols = X.d;
     B2_TRY(make_tmap(&tq, q_filt, op, nq, op_cols, q_pitch, BLOCK_M));
-    // pair mode: each CTA of the pair loads HALF of the 256-row corpus tile (and multicasts it to both)
-    B2_TRY(make_tmap(&tx, X.filt, op, X.n, op_cols, X.filt_pitch, two_cta ? BLOCK_N / 2 : BLOCK_N));
+    // each CTA of a cluster loads 1/cluster of the 256-row corpus tile (and multicasts it to all of them)
+    B2_TRY(make_tmap(&tx, X.filt, op, X.n, op_cols, X.filt_pitch, BLOCK_N / cluster));
     FilterParams p;
     p.xnorm = X.norm2;
     p.cand_score = cand_score;
@@ -966,7 +1056,7 @@ int launch_knn_filter(const MatView& X, const void* q_filt, int64_t q_pitch, int
     p.n = (int32_t)X.n;
     p.num_kb = (int32_t)ceil_div(X.d, kb_elems);
     p.n_mtiles = (int32_t)ceil_div(nq, BLOCK_M);
-    p.n_munits = two_cta ? (p.n_mtiles + 1) / 2 : p.n_mtiles;
+    p.n_munits = cluster > 1 ? (p.n_mtiles + 1) / 2 : p.n_mtiles;
     p.n_ntiles = (int32_t)ceil_div(X.n, BLOCK_N);
     p.tiles_per_split = (int32_t)ceil_div(p.n_ntiles, n_splits);
     p.n_splits = n_splits;
@@ -987,6 +1077,15 @@ int launch_knn_filter(const MatView& X, const void* q_filt, int64_t q_pitch, int
         set_error("internal: bad two-phase schedule (%d whole units of %d)", units_whole, p.n_munits);
         return B2_EINVAL;
     }
+    if (cluster > 2) {
+        // the two CTA pairs of a cluster sweep the same corpus tiles only with an even worker count, an even number of whole
+        // units and an even number of units cut into splits: a surplus unit past the last query tile loads zeros, writes nothing
+        if (workers % 2 != 0 || units_whole % 2 != 0) {
+            set_error("internal: clusters of %d with %d workers and %d whole units", cluster, workers, units_whole);
+            return B2_EINVAL;
+        }
+        p.n_munits += (p.n_munits - units_whole) & 1;
+    }
     const int64_t items = (int64_t)units_whole + (int64_t)(p.n_munits - units_whole) * n_splits;
     if (units_whole > 0 && n_splits > 1) {
         // whole units write split 0 only: the other lists of their queries must read as empty (id -1, bound -inf)
@@ -998,15 +1097,19 @@ int launch_knn_filter(const MatView& X, const void* q_filt, int64_t q_pitch, int
         set_error("internal: L2 filter without row norms");
         return B2_EINVAL;
     }
-    int rc;
-    if (two_cta) {
-        const int pairs = (int)std::min<int64_t>(items, sm_count(device) / 2);
-        rc = launch_two<true>(kp, is_l2, op, tq, tx, p, 2 * pairs, stream);
-    } else {
-        const int grid = (int)std::min<int64_t>(items, sm_count(device));
-        rc = launch_two<false>(kp, is_l2, op, tq, tx, p, grid, stream);
+    if ((cluster != 1 && cluster != 2 && (cluster != FILTER_CL || p.top1)) || workers <= 0) {
+        set_error("internal: bad filter launch (%d workers of %d CTAs)", workers, cluster);
+        return B2_EINVAL;
     }
-    return rc;
+    // workers are CTA pairs in cluster mode; in clusters of four both counts are even, so whole clusters are launched
+    const int grid = (cluster > 1 ? 2 : 1) * (int)std::min<int64_t>(items, workers);
+    if (p.top1)
+        return cluster == 1 ? launch_top1<1>(is_l2, op, tq, tx, p, grid, stream) : launch_top1<2>(is_l2, op, tq, tx, p, grid, stream);
+    switch (cluster) {
+        case 1: return launch_cl<1>(kp, is_l2, op, tq, tx, p, grid, stream);
+        case 2: return launch_cl<2>(kp, is_l2, op, tq, tx, p, grid, stream);
+        default: return launch_cl<FILTER_CL>(kp, is_l2, op, tq, tx, p, grid, stream);
+    }
 }
 
 // query tiles per dealing group of the all-pairs schedule: one per SM, so that one wave of CTAs is one group
@@ -1067,14 +1170,14 @@ int launch_pair_filter(const MatView& X, float thr, int part, int nparts, int32_
     const int grid = two_cta ? 2 * (int)std::min<int64_t>(items, sm_count(device) / 2) : (int)std::min<int64_t>(items, sm_count(device));
     switch (op) {
         case Op::TF32:
-            return two_cta ? launch_cluster(pair_filter_kernel<Op::TF32, true>, grid, PAIR_SMEM, true, tq, tx, p, stream)
-                           : launch_cluster(pair_filter_kernel<Op::TF32, false>, grid, PAIR_SMEM, false, tq, tx, p, stream);
+            return two_cta ? launch_cluster(pair_filter_kernel<Op::TF32, 2>, grid, PAIR_SMEM, 2, tq, tx, p, stream)
+                           : launch_cluster(pair_filter_kernel<Op::TF32, 1>, grid, PAIR_SMEM, 1, tq, tx, p, stream);
         case Op::BF16:
-            return two_cta ? launch_cluster(pair_filter_kernel<Op::BF16, true>, grid, PAIR_SMEM, true, tq, tx, p, stream)
-                           : launch_cluster(pair_filter_kernel<Op::BF16, false>, grid, PAIR_SMEM, false, tq, tx, p, stream);
+            return two_cta ? launch_cluster(pair_filter_kernel<Op::BF16, 2>, grid, PAIR_SMEM, 2, tq, tx, p, stream)
+                           : launch_cluster(pair_filter_kernel<Op::BF16, 1>, grid, PAIR_SMEM, 1, tq, tx, p, stream);
         default:  // Op::F16
-            return two_cta ? launch_cluster(pair_filter_kernel<Op::F16, true>, grid, PAIR_SMEM, true, tq, tx, p, stream)
-                           : launch_cluster(pair_filter_kernel<Op::F16, false>, grid, PAIR_SMEM, false, tq, tx, p, stream);
+            return two_cta ? launch_cluster(pair_filter_kernel<Op::F16, 2>, grid, PAIR_SMEM, 2, tq, tx, p, stream)
+                           : launch_cluster(pair_filter_kernel<Op::F16, 1>, grid, PAIR_SMEM, 1, tq, tx, p, stream);
     }
 }
 
