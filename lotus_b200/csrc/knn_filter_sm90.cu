@@ -16,6 +16,10 @@
 //                    registers, 128 per thread) and runs the epilogue of those rows
 //   K-block = one 64-byte swizzle row (32 bf16 or fp16 / 16 tf32): wgmma k16 (bf16, fp16) or k8 (tf32), two per K-block.
 //   smem ring of NSTAGES x (A 8 KB + B 16 KB), mbarrier full/empty pairs.
+//   Resident query K-blocks (knn filter): the query tile is the same for every corpus tile of an item, so each consumer keeps
+//   its rows of the first FILTER_RES_KB K-blocks in registers (8 per K-block, loaded in the item's first tile) and issues
+//   register-A wgmmas for them; in the item's later tiles those stages carry B only. Per 128 x 256 tile a CTA then pulls
+//   (num_kb - FILTER_RES_KB) x 8 KB of A instead of num_kb x 8 KB (d = 768 bf16: 144 instead of 192 KB).
 //   Clusters of CL CTAs (knn filter over a long corpus: FILTER_CL; k-means assignment, short corpora and dedup: CTA pairs; once
 //   a chunk has CL query tiles): the
 //   schedule's worker is a CTA pair that takes two consecutive query tiles (a query unit); a cluster of four runs two such
@@ -43,6 +47,7 @@ constexpr int BLOCK_N = 256;
 constexpr int WG_M = 64;        // query rows per consumer warpgroup (wgmma M)
 constexpr int KB_BYTES = 64;    // K-block: one SWIZZLE_64B row
 constexpr int KSTEPS = 2;       // wgmma K steps (32 bytes each) per K-block
+constexpr int KB_AREGS = 4 * KSTEPS;  // registers per consumer thread holding one K-block of its warpgroup's 64 query rows
 constexpr int STAGE_A_BYTES = BLOCK_M * KB_BYTES;
 constexpr int STAGE_B_BYTES = BLOCK_N * KB_BYTES;
 constexpr int STAGE_BYTES = STAGE_A_BYTES + STAGE_B_BYTES;
@@ -58,6 +63,9 @@ constexpr int BAR_BYTES = 256;
 // corpus of fewer than FILTER_CL_MIN_NTILES tiles keep CTA pairs (DESIGN §5).
 constexpr int FILTER_CL = 4;
 constexpr int FILTER_CL_MIN_NTILES = 32;
+// K-blocks of its query rows that a knn filter consumer keeps in registers for a whole item (8 per K-block next to the 128
+// accumulators), so that after the item's first tile those stages load only B from L2 (DESIGN §5)
+constexpr int FILTER_RES_KB = 6;
 constexpr int FILTER_MAX_K = 1000;  // largest k served by the filter (finalize keeps min(k + 32, 1024) survivors per query)
 
 // pending (not yet merged) candidates per (query row, set): a flush is triggered once any row holds PEND_FLUSH of them,
@@ -199,12 +207,22 @@ __device__ __forceinline__ void acc_fence(float (&d)[128]) {
 enum class Op { BF16, F16, TF32 };
 __host__ __device__ constexpr int op_bytes(Op op) { return op == Op::TF32 ? 4 : 2; }
 
+// the 128 accumulators of an m64n256 wgmma, as operands %0..%127
+#define B2_WGMMA_D                                                                                                           \
+    "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}"
+#define B2_WGMMA_D_OPS                                                                                                       \
+    "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
 #define B2_WGMMA_64X256(SHAPE_TYPES, IMM_TAIL)                                                                               \
     asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"                                                   \
-                 "wgmma.mma_async.sync.aligned." SHAPE_TYPES " "                                                           \
-                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}" ", %128, %129, p, 1, 1" IMM_TAIL ";\n\t}"                                                          \
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])                                                                                                         \
+                 "wgmma.mma_async.sync.aligned." SHAPE_TYPES " " B2_WGMMA_D ", %128, %129, p, 1, 1" IMM_TAIL ";\n\t}"         \
+                 : B2_WGMMA_D_OPS                                                                                          \
                  : "l"(adesc), "l"(bdesc), "r"(scale_d))
+#define B2_WGMMA_64X256_RS(SHAPE_TYPES, IMM_TAIL)                                                                            \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %133, 0;\n\t"                                                   \
+                 "wgmma.mma_async.sync.aligned." SHAPE_TYPES " " B2_WGMMA_D ", {%128, %129, %130, %131}, %132, p, 1, 1"   \
+                 IMM_TAIL ";\n\t}"                                                                                         \
+                 : B2_WGMMA_D_OPS                                                                                          \
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(scale_d))
 
 // D[64 x 256] (+)= A[64 x K] . B[256 x K]^T, both K-major in shared memory; scale_d == 0 overwrites D
 template <Op OP>
@@ -217,7 +235,53 @@ __device__ __forceinline__ void wgmma_64x256(float (&d)[128], uint64_t adesc, ui
         B2_WGMMA_64X256("m64n256k16.f32.bf16.bf16", ", 0, 0");
     }
 }
+// The same product with A from registers: a[0..3] is the warp's 16-row slice of one K step in the mma fragment layout
+// (load_a_frag); B stays in shared memory. Register A takes no transpose immediate, only B's.
+template <Op OP>
+__device__ __forceinline__ void wgmma_64x256_rs(float (&d)[128], const uint32_t* a, uint64_t bdesc, uint32_t scale_d) {
+    if constexpr (OP == Op::TF32) {
+        B2_WGMMA_64X256_RS("m64n256k8.f32.tf32.tf32", "");
+    } else if constexpr (OP == Op::F16) {
+        B2_WGMMA_64X256_RS("m64n256k16.f32.f16.f16", ", 0");
+    } else {  // Op::BF16
+        B2_WGMMA_64X256_RS("m64n256k16.f32.bf16.bf16", ", 0");
+    }
+}
+#undef B2_WGMMA_64X256_RS
 #undef B2_WGMMA_64X256
+#undef B2_WGMMA_D_OPS
+#undef B2_WGMMA_D
+
+// Register-A fragment of one K-block: a[4k..4k+3] feed K step k of wgmma_64x256_rs. `slice` is the shared address of the
+// consumer warpgroup's 64 query rows in a landed stage (K-major, 64-byte rows, SWIZZLE_64B: the 16-byte chunk c of row r
+// sits at chunk c ^ ((r >> 1) & 3), r counted from a 512-byte-aligned base). Warp w of the warpgroup holds rows 16 w .. 16 w + 15.
+//   2-byte operands: register j of a step holds row (lane / 4) + 8 (j & 1), elements 2 (lane % 4) + {0, 1} + 8 (j >> 1):
+//                    one ldmatrix.x4, lane l addressing row l % 8 of the 8 x 8 matrix l / 8.
+//   tf32:            register j holds row (lane / 4) + 8 (j & 1), element (lane % 4) + 4 (j >> 1): one 4-byte load each.
+template <Op OP>
+__device__ __forceinline__ void load_a_frag(uint32_t (&a)[KB_AREGS], uint32_t slice) {
+    const int lane = threadIdx.x & 31;
+    const int r0 = ((threadIdx.x >> 5) & 3) * 16;
+    auto chunk_addr = [slice](int r, int c) { return slice + (uint32_t)(r * KB_BYTES + ((c ^ ((r >> 1) & 3)) << 4)); };
+#pragma unroll
+    for (int k = 0; k < KSTEPS; ++k) {
+        uint32_t* f = a + 4 * k;
+        if constexpr (OP == Op::TF32) {
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                const uint32_t addr = chunk_addr(r0 + (lane >> 2) + 8 * (j & 1), 2 * k + (j >> 1)) + 4 * (lane & 3);
+                asm volatile("ld.shared.b32 %0, [%1];" : "=r"(f[j]) : "r"(addr) : "memory");
+            }
+        } else {
+            const int m = lane >> 3;
+            const uint32_t addr = chunk_addr(r0 + 8 * (m & 1) + (lane & 7), 2 * k + (m >> 1));
+            asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+                         : "=r"(f[0]), "=r"(f[1]), "=r"(f[2]), "=r"(f[3])
+                         : "r"(addr)
+                         : "memory");
+        }
+    }
+}
 
 struct FilterParams {
     const float* xnorm;  // [n], L2 only
@@ -322,7 +386,9 @@ __device__ __forceinline__ void item_range(const FilterParams& p, const Sched& s
 // loads its own query rows and 1/CL of the corpus tile, multicast to every CTA; every CTA's full barrier counts a whole stage.
 // A piece of BLOCK_N / CL rows is a whole number of 512-byte SWIZZLE_64B periods, so the pieces tile the B stage exactly as
 // one full-tile box would.
-template <Op OP, int NSTAGES, int CL>
+// The first RES_KB K-blocks of the query tile stay in the consumers' registers for the whole item (mma_tile), so after the
+// item's first tile their stages carry B only. A is never multicast, so only this CTA's expected byte count changes.
+template <Op OP, int NSTAGES, int CL, int RES_KB>
 __device__ __forceinline__ void producer_loop(const CUtensorMap* tmap_q, const CUtensorMap* tmap_x, const FilterParams& p,
                                               const Ring& r, const Sched& sc) {
     constexpr int KB_ELEMS = KB_BYTES / op_bytes(OP);
@@ -337,8 +403,9 @@ __device__ __forceinline__ void producer_loop(const CUtensorMap* tmap_q, const C
                 mbar_wait(&r.empty_bar[stage], phase ^ 1);
                 uint8_t* sa = r.stage_base + stage * STAGE_BYTES;
                 uint8_t* sb = sa + STAGE_A_BYTES;
-                mbar_arrive_expect_tx(&r.full_bar[stage], STAGE_BYTES);
-                tma_load_2d(sa, tmap_q, &r.full_bar[stage], kb * KB_ELEMS, m_tile * BLOCK_M);
+                const bool a_resident = t != t0 && kb < RES_KB;
+                mbar_arrive_expect_tx(&r.full_bar[stage], a_resident ? STAGE_B_BYTES : STAGE_BYTES);
+                if (!a_resident) tma_load_2d(sa, tmap_q, &r.full_bar[stage], kb * KB_ELEMS, m_tile * BLOCK_M);
                 if constexpr (CL > 1)
                     tma_load_2d_multicast(sb + sc.cta * (STAGE_B_BYTES / CL), tmap_x, &r.full_bar[stage], kb * KB_ELEMS,
                                           t * BLOCK_N + sc.cta * (BLOCK_N / CL), (uint16_t)((1u << CL) - 1));
@@ -372,19 +439,15 @@ __device__ __forceinline__ void release_stage(const Ring& r, int s, int cta) {
 
 // Consumer warpgroup g: acc = (query rows 64g..64g+63 of the stage's A tile) . (the 256 corpus rows)^T over all K-blocks of
 // one corpus tile. One wgmma group per K-block; a stage is released as soon as the group that read it has retired.
-template <Op OP, int NSTAGES, int CL>
-__device__ __forceinline__ void mma_tile(float (&acc)[128], const Ring& r, int num_kb, int g, int cta, int& stage, uint32_t& phase) {
+// K-blocks kb < RES_KB take A from `afrag`, which holds them for the whole item: the item's first tile (load_a) fills it from
+// the landed stages, later tiles find no A in those stages (producer_loop). The rest read A from shared memory. The operands
+// and the K order are the same either way, so are the accumulators.
+template <Op OP, int NSTAGES, int CL, int RES_KB>
+__device__ __forceinline__ void mma_tile(float (&acc)[128], uint32_t (&afrag)[RES_KB > 0 ? RES_KB : 1][KB_AREGS], bool load_a,
+                                         const Ring& r, int num_kb, int g, int cta, int& stage, uint32_t& phase) {
     const uint32_t a_off = (uint32_t)(g * WG_M * KB_BYTES);
     int prev = -1;
-    for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait_spin(&r.full_bar[stage], phase);
-        const uint32_t sa = smem_u32(r.stage_base + stage * STAGE_BYTES);
-        const uint64_t adesc = make_sw64_desc(sa + a_off);
-        const uint64_t bdesc = make_sw64_desc(sa + STAGE_A_BYTES);
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < KSTEPS; ++k)  // +32 bytes per K step inside the 64-byte swizzle row (16 B units)
-            wgmma_64x256<OP>(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (kb | k) != 0 ? 1u : 0u);
+    auto retire = [&]() {
         wgmma_commit();
         if (prev >= 0) {
             wgmma_wait<1>();
@@ -395,6 +458,31 @@ __device__ __forceinline__ void mma_tile(float (&acc)[128], const Ring& r, int n
             stage = 0;
             phase ^= 1;
         }
+    };
+#pragma unroll
+    for (int kb = 0; kb < RES_KB; ++kb) {
+        if (kb < num_kb) {
+            mbar_wait_spin(&r.full_bar[stage], phase);
+            const uint32_t sa = smem_u32(r.stage_base + stage * STAGE_BYTES);
+            if (load_a) load_a_frag<OP>(afrag[kb], sa + a_off);
+            const uint64_t bdesc = make_sw64_desc(sa + STAGE_A_BYTES);
+            wgmma_fence();  // orders the fragment writes (and the accumulators') before the wgmmas that read them
+#pragma unroll
+            for (int k = 0; k < KSTEPS; ++k)
+                wgmma_64x256_rs<OP>(acc, afrag[kb] + 4 * k, bdesc + (uint64_t)(2 * k), (kb | k) != 0 ? 1u : 0u);
+            retire();
+        }
+    }
+    for (int kb = RES_KB; kb < num_kb; ++kb) {
+        mbar_wait_spin(&r.full_bar[stage], phase);
+        const uint32_t sa = smem_u32(r.stage_base + stage * STAGE_BYTES);
+        const uint64_t adesc = make_sw64_desc(sa + a_off);
+        const uint64_t bdesc = make_sw64_desc(sa + STAGE_A_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < KSTEPS; ++k)  // +32 bytes per K step inside the 64-byte swizzle row (16 B units)
+            wgmma_64x256<OP>(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (kb | k) != 0 ? 1u : 0u);
+        retire();
     }
     wgmma_wait<0>();
     acc_fence(acc);
@@ -557,6 +645,7 @@ knn_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
     constexpr int KPH = KP / 2;  // candidates kept per (row, set)
     static_assert(KPH % 4 == 0, "list length must allow float4 write-out");
     constexpr int LSET = list_set_stride(KPH);
+    constexpr int RES_KB = FILTER_RES_KB;
 
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = align_smem(smem_raw);
@@ -573,7 +662,7 @@ knn_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
 
     if (warp < 4) {
         setmaxnreg_dec<40>();
-        if (threadIdx.x == 0) producer_loop<OP, NSTAGES, CL>(&tmap_q, &tmap_x, p, ring, sc);
+        if (threadIdx.x == 0) producer_loop<OP, NSTAGES, CL, RES_KB>(&tmap_q, &tmap_x, p, ring, sc);
     } else {
         setmaxnreg_inc<232>();
         // ===================== consumer warpgroup g: wgmma of 64 query rows, streaming top-KPH per (row, set) ==========
@@ -591,6 +680,7 @@ knn_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
         int stage = 0;
         uint32_t phase = 0;
         float acc[128];
+        uint32_t afrag[RES_KB][KB_AREGS];  // the query tile's first RES_KB K-blocks, loaded in each item's first tile
         for (int item = sc.worker; item < n_items; item += sc.n_workers) {
             int m_tile, split, t0, t1;
             item_range<CL>(p, sc, item, m_tile, split, t0, t1);
@@ -610,7 +700,7 @@ knn_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
             // lane fr + 8h + 16s
             float gthr[2][2] = {{-INFINITY, -INFINITY}, {-INFINITY, -INFINITY}};
             for (int t = t0; t < t1; ++t) {
-                mma_tile<OP, NSTAGES, CL>(acc, ring, p.num_kb, g, sc.cta, stage, phase);
+                mma_tile<OP, NSTAGES, CL, RES_KB>(acc, afrag, t == t0, ring, p.num_kb, g, sc.cta, stage, phase);
                 const int col0 = t * BLOCK_N;
                 const int ncols = min(BLOCK_N, p.n - col0);
 #pragma unroll
@@ -717,7 +807,7 @@ pair_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_cons
     const Sched sc = make_sched<CL>();
     if (warp < 4) {
         setmaxnreg_dec<40>();
-        if (threadIdx.x == 0) producer_loop<OP, PAIR_STAGES, CL>(&tmap_q, &tmap_x, p, ring, sc);
+        if (threadIdx.x == 0) producer_loop<OP, PAIR_STAGES, CL, 0>(&tmap_q, &tmap_x, p, ring, sc);
     } else {
         setmaxnreg_inc<232>();
         const int g = (warp >> 2) - 1;
@@ -726,12 +816,13 @@ pair_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_cons
         int stage = 0;
         uint32_t phase = 0;
         float acc[128];
+        uint32_t no_afrag[1][KB_AREGS];  // every K-block reads A from shared memory
         for (int item = sc.worker; item < n_items; item += sc.n_workers) {
             int m_tile, split, t0, t1;
             item_range<CL>(p, sc, item, m_tile, split, t0, t1);
             const int gi0 = m_tile * BLOCK_M + g * WG_M + wq * 16 + (lane >> 2);  // global rows gi0 and gi0 + 8 of this lane
             for (int t = t0; t < t1; ++t) {
-                mma_tile<OP, PAIR_STAGES, CL>(acc, ring, p.num_kb, g, sc.cta, stage, phase);
+                mma_tile<OP, PAIR_STAGES, CL, 0>(acc, no_afrag, false, ring, p.num_kb, g, sc.cta, stage, phase);
                 const int col0 = t * BLOCK_N + 2 * (lane & 3);
                 float mx = acc[0];
 #pragma unroll
