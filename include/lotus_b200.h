@@ -61,6 +61,15 @@ extern "C" {
  * component of magnitude >= 65520 sends that query to the exact dense path); the reported scores always use the
  * query as given. */
 enum { B2_F32 = 0, B2_BF16 = 1, B2_F16 = 2 };
+/* B2_I8: signed 8-bit integers (two's complement), e.g. quantized embeddings. An int8 index with int8 queries is filtered on
+ * the int8 tensor cores (s8 x s8 -> s32, exact integer accumulation), so its results are those of the fp32 upcast of the
+ * stored values. fp32 / bf16 / fp16 queries on an int8 index are filtered against an fp16 copy of the rows (exact), built
+ * on the first such search and kept with the handle (2 more bytes per element). int8 queries on the other indexes are
+ * widened exactly. An int8 index needs d < 2^17 (the s32 accumulator range), and d < 2^15 with B2_METRIC_L2 (the filter
+ * forms 2 <q, x> - |x|^2 in int32). b2_threshold_pairs runs the int8 pair filter; its threshold is in units of int8 inner
+ * products. k-means runs on an fp16 copy of the rows (exact), made on the first k-means call and kept with the handle.
+ * The code is kept apart from the floating-point types. */
+enum { B2_I8 = 8 };
 /* metrics; numeric values match faiss.METRIC_INNER_PRODUCT / faiss.METRIC_L2 */
 enum { B2_METRIC_IP = 0, B2_METRIC_L2 = 1 };
 

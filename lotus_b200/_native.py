@@ -12,7 +12,8 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libb2lotus.so")
 
 F32, BF16, F16 = 0, 1, 2
-DTYPES = (F32, BF16, F16)
+DTYPES = (F32, BF16, F16)  # the floating-point types
+I8 = 8  # signed 8-bit integers (B2_I8), kept apart from the floating-point codes
 METRIC_IP, METRIC_L2 = 0, 1
 OK, EINVAL, ENODEV, ECUDA, ENOMEM, ERANGE = 0, -1, -2, -3, -4, -5
 
@@ -180,9 +181,11 @@ def bf16_bits_to_f32(b: np.ndarray) -> np.ndarray:
 
 def storage_dtype(code: int) -> np.dtype:
     """numpy dtype of a matrix's elements as the C-ABI holds them: float32, bfloat16 bit patterns (uint16; numpy has no
-    bfloat16) or float16."""
+    bfloat16), float16 or int8."""
     if code == F32:
         return np.dtype(np.float32)
+    if code == I8:
+        return np.dtype(np.int8)
     if code == BF16:
         return np.dtype(np.uint16)
     if code == F16:
@@ -200,6 +203,8 @@ def stored_to_f32(a: np.ndarray, code: int) -> np.ndarray:
     if code == F16:
         a = np.ascontiguousarray(a)
         return (a.view(np.float16) if a.dtype == np.uint16 else a.astype(np.float16, copy=False)).astype(np.float32)
+    if code == I8:
+        return np.ascontiguousarray(a, dtype=np.int8).astype(np.float32)
     raise ValueError(f"unknown element type code {code}")
 
 

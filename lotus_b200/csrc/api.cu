@@ -51,6 +51,8 @@ int build_view(const void* store, int64_t n, int d, int dtype, DevBuf& filt_pad,
     }
     v.filt16 = nullptr;
     v.filt16_pitch = 0;
+    v.filt_f16 = nullptr;
+    v.filt_f16_pitch = 0;
     static const bool bf16_first = [] { const char* e = getenv("B2_F32_BF16_FIRST"); return e ? atoi(e) != 0 : true; }();
     if (filt16 && dtype == B2_F32 && bf16_first && n >= 4096) {
         v.filt16_pitch = round_up(d, 8);
@@ -58,9 +60,15 @@ int build_view(const void* store, int64_t n, int d, int dtype, DevBuf& filt_pad,
         B2_TRY(launch_convert_pad(store, dtype, n, d, filt16->p, B2_BF16, v.filt16_pitch, st));
         v.filt16 = filt16->p;
     }
-    B2_TRY(norm2.ensure((size_t)std::max<int64_t>(n, 1) * sizeof(float)));
+    // int8 stores keep the exact integer norms after the fp32 ones (int8 L2 filter epilogue)
+    B2_TRY(norm2.ensure((size_t)std::max<int64_t>(n, 1) * (dtype == B2_I8 ? 2 : 1) * sizeof(float)));
     B2_TRY(scalar.ensure(64));
     B2_TRY(launch_row_norms(store, dtype, n, d, norm2.as<float>(), scalar.as<float>(), st));
+    v.norm2_i8 = nullptr;
+    if (dtype == B2_I8) {
+        v.norm2_i8 = reinterpret_cast<const int32_t*>(norm2.as<float>() + std::max<int64_t>(n, 1));
+        B2_TRY(launch_row_norms_i8(store, n, d, const_cast<int32_t*>(v.norm2_i8), st));
+    }
     float mx = 0.f;
     B2_CUDA(cudaMemcpyAsync(&mx, scalar.p, sizeof(float), cudaMemcpyDeviceToHost, st));
     B2_CUDA(cudaStreamSynchronize(st));
@@ -74,7 +82,9 @@ int build_view(const void* store, int64_t n, int d, int dtype, DevBuf& filt_pad,
 //   bf16 wgmma: fp32 values are rounded to bf16 (2^-8); fp16 values (11-bit significand) are rounded too, also 2^-8.
 //   fp16 wgmma: fp32 and bf16 values are rounded to fp16 (2^-11 relative, plus the absolute term of filter_abs_eps for the
 //   subnormal range). bf16 values that are fp16-normal would be exact, but a bf16 value can lie outside fp16's range.
+//   int8 values (|v| <= 128) are exact in every filter type; the int8 wgmma only ever sees int8 operands.
 static double operand_rel_err(int dtype, int filt_dtype) {
+    if (dtype == B2_I8 || filt_dtype == B2_I8) return 0.0;
     switch (filt_dtype) {
         case B2_F32: return dtype == B2_F32 ? 9.765625e-4 : 0.0;
         case B2_BF16: return dtype == B2_BF16 ? 0.0 : 3.90625e-3;
@@ -88,7 +98,9 @@ float filter_rel_eps(int store_dtype, int filt_dtype, int q_dtype, int d) {
     // (truncated) ulp of the running magnitude; (d + 64) * 2^-23 is generous. tests/test_gpu_filter_lists.py checks every
     // list entry against this bound in its per-row form (|x| of the row, not max |x|) and pins the formula; the largest
     // measured |err| is 0.66 rel_eps |q| |x| (DESIGN.md §2).
-    const double acc = (double)(d + 64) * 1.1920929e-7;
+    // The int8 wgmma accumulates exactly in s32; its one error is the conversion of the sum s to fp32, at most 2^-24 |s| <=
+    // 2^-24 |q| |x| (and none while |s| < 2^24).
+    const double acc = filt_dtype == B2_I8 ? 5.9604644775390625e-8 : (double)(d + 64) * 1.1920929e-7;
     // relative representation error of the corpus / query operand seen by the MMA
     const double ex = operand_rel_err(store_dtype, filt_dtype), eq = operand_rel_err(q_dtype, filt_dtype);
     return (float)(acc + ex + eq + ex * eq + 1e-6);
@@ -101,7 +113,8 @@ float filter_rel_eps(int store_dtype, int filt_dtype, int q_dtype, int d) {
 // of two rounded sides would need more than this.)
 float filter_abs_eps(int store_dtype, int filt_dtype, int q_dtype, int d) {
     if (filt_dtype != B2_F16) return 0.f;
-    const int rounded = (store_dtype != B2_F16 ? 1 : 0) + (q_dtype != B2_F16 ? 1 : 0);
+    auto exact = [](int dt) { return dt == B2_F16 || dt == B2_I8; };  // int8 values are exact in fp16
+    const int rounded = (exact(store_dtype) ? 0 : 1) + (exact(q_dtype) ? 0 : 1);
     return (float)(rounded * 2.9802322387695312e-8 * sqrt((double)d) * (1.0 + 1e-6));
 }
 
@@ -146,6 +159,15 @@ int plan_filter(const MatView& X_in, const void* q, int q_dtype, int64_t nq, int
         p.X.filt = X_in.filt16;
         p.X.filt_pitch = X_in.filt16_pitch;
         p.X.filt_dtype = B2_BF16;
+    }
+    if (X_in.dtype == B2_I8 && q_dtype != B2_I8) {  // floating-point queries on an int8 store: its fp16 copy (exact)
+        if (!X_in.filt_f16 && model_sms <= 0) {
+            set_error("internal: int8 store without its fp16 copy");
+            return B2_EINVAL;
+        }
+        p.X.filt = X_in.filt_f16;
+        p.X.filt_pitch = X_in.filt_f16_pitch;
+        p.X.filt_dtype = B2_F16;
     }
     const MatView& X = p.X;
     p.kp = p.two_level ? kp16 : filter_kp_for_k(k);
@@ -328,11 +350,38 @@ int gather_rows_checked(const void* x, int dtype, int d, const int64_t* ids, int
     return B2_OK;
 }
 
+// The fp16 copy of an int8 view that fp32 / bf16 / fp16 queries are filtered against, made once and kept in `buf`.
+static int ensure_f16_copy(MatView& v, DevBuf& buf, cudaStream_t st) {
+    if (v.dtype != B2_I8 || v.filt_f16) return B2_OK;
+    v.filt_f16_pitch = round_up(v.d, tma_align_elems(B2_F16));
+    B2_TRY(buf.ensure((size_t)std::max<int64_t>(v.n, 1) * v.filt_f16_pitch * 2));
+    B2_TRY(launch_convert_pad(v.store, B2_I8, v.n, v.d, buf.p, B2_F16, v.filt_f16_pitch, st));
+    v.filt_f16 = buf.p;
+    return B2_OK;
+}
+
+// Queries as the store's pipeline takes them. int8 queries on a floating-point store are widened exactly, to fp16 on an fp16
+// store and to bf16 otherwise, so that the store's own finalize kernel serves them and every filter level sees an operand of
+// no representation error (bf16 is exact in tf32 and on an fp32 store's bf16 first level alike); other queries on an int8
+// store need its fp16 copy.
+static int adapt_queries(b2_index* idx, const void*& q, int32_t& q_dtype, int64_t nq, cudaStream_t st) {
+    if (q_dtype == B2_I8 && idx->dtype != B2_I8 && nq > 0) {
+        const int wide = idx->dtype == B2_F16 ? B2_F16 : B2_BF16;
+        B2_TRY(idx->q_wide.ensure((size_t)nq * idx->d * 2));
+        B2_TRY(launch_convert_pad(q, B2_I8, nq, idx->d, idx->q_wide.p, wide, idx->d, st));
+        q = idx->q_wide.p;
+        q_dtype = wide;
+    }
+    if (q_dtype != B2_I8) B2_TRY(ensure_f16_copy(idx->view, idx->filt_f16, st));
+    return B2_OK;
+}
+
 // searchable view for an ids subset (faiss_vs.py:57-64: temporary index over vecs[ids])
-static int build_subset(b2_index* idx, const int64_t* ids_dev, int64_t m, MatView& sub, cudaStream_t st) {
+static int build_subset(b2_index* idx, const int64_t* ids_dev, int64_t m, int q_dtype, MatView& sub, cudaStream_t st) {
     B2_TRY(idx->sub_store.ensure((size_t)std::max<int64_t>(m, 1) * idx->d * esize(idx->dtype)));
     B2_TRY(gather_rows_checked(idx->store.p, idx->dtype, idx->d, ids_dev, m, idx->n, idx->sub_store.p, idx->scalar, st));
-    return build_view(idx->sub_store.p, m, idx->d, idx->dtype, idx->sub_filt, idx->sub_norm2, idx->scalar, sub, st, &idx->sub_filt16);
+    B2_TRY(build_view(idx->sub_store.p, m, idx->d, idx->dtype, idx->sub_filt, idx->sub_norm2, idx->scalar, sub, st, &idx->sub_filt16));
+    return q_dtype != B2_I8 ? ensure_f16_copy(sub, idx->sub_filt_f16, st) : B2_OK;
 }
 
 // Runs body(lo, hi) over [0, count) in chunks of 2^20 elements on up to 16 host threads.
@@ -357,7 +406,29 @@ static void for_each_chunk(int64_t count, const Body& body) {
 
 }  // namespace b2
 
+namespace b2 {
+// k-means over an int8 index runs on an fp16 twin of it (same rows, exact in fp16), made on the first k-means call and kept
+// with the handle: the existing fp16 k-means path (fp16 TOP1 filter, fp16 accumulate) then serves int8 points unchanged
+int kmeans_view(b2_index* idx, b2_index** out) {
+    *out = idx;
+    if (idx->dtype != B2_I8) return B2_OK;
+    if (!idx->f16_twin) {
+        DevBuf tmp;
+        B2_TRY(tmp.ensure((size_t)std::max<int64_t>(idx->n, 1) * idx->d * 2));
+        B2_TRY(launch_convert_pad(idx->store.p, B2_I8, idx->n, idx->d, tmp.p, B2_F16, idx->d, idx->stream));
+        B2_CUDA(cudaStreamSynchronize(idx->stream));
+        b2_index* t = nullptr;
+        B2_TRY(b2_index_create(tmp.p, idx->n, idx->d, B2_F16, idx->metric, idx->device, 1, &t));
+        B2_CUDA(cudaStreamSynchronize(t->stream));
+        idx->f16_twin = t;
+    }
+    *out = idx->f16_twin;
+    return B2_OK;
+}
+}  // namespace b2
+
 b2_index::~b2_index() {
+    if (f16_twin) b2_index_free(f16_twin);
     if (ev0) cudaEventDestroy(ev0);
     if (ev1) cudaEventDestroy(ev1);
     if (stream) cudaStreamDestroy(stream);
@@ -392,7 +463,12 @@ int b2_index_create(const void* x, int64_t n, int32_t d, int32_t dtype, int32_t 
     if (!out) { set_error("out is NULL"); return B2_EINVAL; }
     *out = nullptr;
     if (n < 0 || d <= 0 || (n > 0 && !x)) { set_error("bad matrix shape n=%lld d=%d", (long long)n, d); return B2_EINVAL; }
-    if (!dtype_valid(dtype)) { set_error("dtype must be B2_F32, B2_BF16 or B2_F16"); return B2_EINVAL; }
+    if (!dtype_valid(dtype)) { set_error("dtype must be B2_F32, B2_BF16, B2_F16 or B2_I8"); return B2_EINVAL; }
+    if (dtype == B2_I8 && d > I8_MAX_D) { set_error("an int8 index needs d < 2^17 (got %d): its s32 accumulators would overflow", d); return B2_EINVAL; }
+    if (dtype == B2_I8 && metric == B2_METRIC_L2 && d > I8_L2_MAX_D) {
+        set_error("an int8 L2 index needs d < 2^15 (got %d): 2 <q, x> - |x|^2 would overflow int32", d);
+        return B2_EINVAL;
+    }
     if (metric != B2_METRIC_IP && metric != B2_METRIC_L2) { set_error("metric must be B2_METRIC_IP or B2_METRIC_L2"); return B2_EINVAL; }
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
@@ -455,7 +531,7 @@ float b2_last_filter_ms(const b2_index* idx) { return idx ? idx->last_filter_ms 
 static int check_search_args(b2_index* idx, const void* q, int64_t nq, int32_t q_dtype, int32_t k) {
     if (!idx) { set_error("Index not loaded"); return B2_EINVAL; }
     if (nq < 0 || (nq > 0 && !q)) { set_error("bad query batch"); return B2_EINVAL; }
-    if (!dtype_valid(q_dtype)) { set_error("q_dtype must be B2_F32, B2_BF16 or B2_F16"); return B2_EINVAL; }
+    if (!dtype_valid(q_dtype)) { set_error("q_dtype must be B2_F32, B2_BF16, B2_F16 or B2_I8"); return B2_EINVAL; }
     if (k <= 0) { set_error("k must be positive (got %d)", k); return B2_EINVAL; }
     if (k > dense_max_k()) { set_error("k=%d is not supported (max %d)", k, dense_max_k()); return B2_ERANGE; }
     return B2_OK;
@@ -468,10 +544,11 @@ int b2_index_search_dev(b2_index* idx, const void* q_dev, int64_t nq, int32_t q_
     if (!out_scores_dev || !out_idx_dev) { set_error("output buffers are NULL"); return B2_EINVAL; }
     DeviceGuard guard(idx->device);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    B2_TRY(adapt_queries(idx, q_dev, q_dtype, nq, st));
     if (ids_dev) {
         if (n_ids < 0) { set_error("n_ids < 0"); return B2_EINVAL; }
         MatView sub;
-        B2_TRY(build_subset(idx, ids_dev, n_ids, sub, st));
+        B2_TRY(build_subset(idx, ids_dev, n_ids, q_dtype, sub, st));
         B2_TRY(search_core(idx, sub, idx->metric, q_dev, q_dtype, nq, k, ids_dev, 0, out_scores_dev, out_idx_dev, st));
     } else {
         B2_TRY(search_core(idx, idx->view, idx->metric, q_dev, q_dtype, nq, k, nullptr, id_offset, out_scores_dev, out_idx_dev, st));
@@ -492,6 +569,8 @@ int b2_index_search(b2_index* idx, const void* q, int64_t nq, int32_t q_dtype, i
     B2_TRY(idx->out_sc.ensure((size_t)nq * k * sizeof(float)));
     B2_TRY(idx->out_id.ensure((size_t)nq * k * sizeof(int64_t)));
     B2_CUDA(cudaMemcpyAsync(idx->q_in.p, q, qbytes, cudaMemcpyHostToDevice, st));
+    const void* q_dev = idx->q_in.p;
+    B2_TRY(adapt_queries(idx, q_dev, q_dtype, nq, st));
     const int64_t* ids_dev = nullptr;
     if (ids) {
         if (n_ids < 0) { set_error("n_ids < 0"); return B2_EINVAL; }
@@ -505,10 +584,10 @@ int b2_index_search(b2_index* idx, const void* q, int64_t nq, int32_t q_dtype, i
     }
     if (ids_dev) {
         MatView sub;
-        B2_TRY(build_subset(idx, ids_dev, n_ids, sub, st));
-        B2_TRY(search_core(idx, sub, idx->metric, idx->q_in.p, q_dtype, nq, k, ids_dev, 0, idx->out_sc.as<float>(), idx->out_id.as<int64_t>(), st));
+        B2_TRY(build_subset(idx, ids_dev, n_ids, q_dtype, sub, st));
+        B2_TRY(search_core(idx, sub, idx->metric, q_dev, q_dtype, nq, k, ids_dev, 0, idx->out_sc.as<float>(), idx->out_id.as<int64_t>(), st));
     } else {
-        B2_TRY(search_core(idx, idx->view, idx->metric, idx->q_in.p, q_dtype, nq, k, nullptr, 0, idx->out_sc.as<float>(),
+        B2_TRY(search_core(idx, idx->view, idx->metric, q_dev, q_dtype, nq, k, nullptr, 0, idx->out_sc.as<float>(),
                            idx->out_id.as<int64_t>(), st));
     }
     B2_CUDA(cudaMemcpyAsync(out_scores, idx->out_sc.p, (size_t)nq * k * sizeof(float), cudaMemcpyDeviceToHost, st));
@@ -540,6 +619,7 @@ int b2_index_search_packed_dev(b2_index* idx, const void* q_dev, int64_t nq, int
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     B2_TRY(idx->out_sc.ensure((size_t)nq * k * sizeof(float)));
     B2_TRY(idx->out_id.ensure((size_t)nq * k * sizeof(int64_t)));
+    B2_TRY(adapt_queries(idx, q_dev, q_dtype, nq, st));
     B2_TRY(search_core(idx, idx->view, idx->metric, q_dev, q_dtype, nq, k, nullptr, 0, idx->out_sc.as<float>(), idx->out_id.as<int64_t>(), st));
     B2_TRY(launch_pack_topk(idx->out_sc.as<float>(), idx->out_id.as<int64_t>(), nq * (int64_t)k, out_packed_dev, st));
     B2_CUDA(cudaStreamSynchronize(st));
@@ -560,6 +640,7 @@ int b2_index_search_stage1_dev(b2_index* idx, const void* q_dev, int64_t nq, int
     if (!lower_dev || j <= 0) { set_error("bad stage-1 arguments"); return B2_EINVAL; }
     DeviceGuard guard(idx->device);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    B2_TRY(adapt_queries(idx, q_dev, q_dtype, nq, st));
     b2_index::Staged& sg = idx->staged;
     sg = b2_index::Staged();
     sg.active = true;
@@ -704,12 +785,19 @@ int b2_debug_filter_lists(b2_index* idx, const void* q, int64_t nq, int32_t q_dt
     MatView X = idx->view;
     if (level == 1 || top1) X.filt16 = nullptr;  // the second level drops the bf16 copy; the k-means centroid view has none
     const size_t qbytes = (size_t)nq * idx->d * esize(q_dtype);
+    const void* q_dev = nullptr;
     if (lists) {
         B2_TRY(idx->q_in.ensure(qbytes));
         B2_CUDA(cudaMemcpyAsync(idx->q_in.p, q, qbytes, cudaMemcpyHostToDevice, st));
+        q_dev = idx->q_in.p;
+        B2_TRY(adapt_queries(idx, q_dev, q_dtype, nq, st));
+    } else if (q_dtype != B2_I8) {
+        B2_TRY(ensure_f16_copy(idx->view, idx->filt_f16, st));
     }
+    X.filt_f16 = idx->view.filt_f16;
+    X.filt_f16_pitch = idx->view.filt_f16_pitch;
     FilterPlan p;
-    B2_TRY(plan_filter(X, lists ? idx->q_in.p : nullptr, q_dtype, nq, k, top1 != 0, idx->device, p));
+    B2_TRY(plan_filter(X, q_dev, q_dtype, nq, k, top1 != 0, idx->device, p));
     const FilterChunk c = p.use_filter ? p.chunks[0] : FilterChunk();
     plan[0] = p.use_filter ? 1 : 0;
     plan[1] = p.use_filter ? p.kp : 0;

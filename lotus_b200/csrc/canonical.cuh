@@ -33,11 +33,20 @@ __device__ __forceinline__ void unpack4(const uint2& t, float (&o)[4]) {
     }
 }
 
+// four int8 elements packed in a 32-bit word (element order = memory order), as fp32
+__device__ __forceinline__ void unpack4_i8(uint32_t w, float (&o)[4]) {
+#pragma unroll
+    for (int e = 0; e < 4; ++e) o[e] = (float)(int8_t)(w >> (8 * e));
+}
+
 // 4 consecutive elements of group g of a row (zero beyond d). `vec` = row start is 4-element aligned.
+template <bool WITH_I8 = false>
 __device__ __forceinline__ void load_group(const void* row, int dtype, int g, int d, bool vec, float (&o)[4]) {
     const int i0 = g * 4;
     if (vec) {
-        if (dtype == B2_F32) {
+        if (WITH_I8 && dtype == B2_I8) {
+            unpack4_i8(__ldg(reinterpret_cast<const uint32_t*>(row) + g), o);
+        } else if (dtype == B2_F32) {
             const float4 t = __ldg(reinterpret_cast<const float4*>(row) + g);
             o[0] = t.x; o[1] = t.y; o[2] = t.z; o[3] = t.w;
         } else if (dtype == B2_BF16) {
@@ -47,18 +56,18 @@ __device__ __forceinline__ void load_group(const void* row, int dtype, int g, in
         }
     } else {
 #pragma unroll
-        for (int e = 0; e < 4; ++e) o[e] = (i0 + e < d) ? elem_f32(row, dtype, (size_t)(i0 + e)) : 0.f;
+        for (int e = 0; e < 4; ++e) o[e] = (i0 + e < d) ? elem_f32<WITH_I8>(row, dtype, (size_t)(i0 + e)) : 0.f;
     }
 }
 
 // canonical partial (this lane's share) of <q, x> or ||q - x||^2; q lives in shared memory as fp32
-template <bool IS_L2>
+template <bool IS_L2, bool WITH_I8 = false>
 __device__ __forceinline__ double canonical_partial(const float* q_s, const void* row, int dtype, int d, bool vec, int lane) {
     double acc = 0.0;
     const int ngroups = (d + 3) >> 2;
     for (int g = lane; g < ngroups; g += 32) {
         float x[4];
-        load_group(row, dtype, g, d, vec, x);
+        load_group<WITH_I8>(row, dtype, g, d, vec, x);
         const float4 q4 = *reinterpret_cast<const float4*>(q_s + 4 * g);
         const float qq[4] = {q4.x, q4.y, q4.z, q4.w};
 #pragma unroll

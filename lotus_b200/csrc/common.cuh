@@ -79,11 +79,20 @@ __host__ __device__ __forceinline__ float best_first_unkey(uint32_t k, int metri
 }
 
 // ---- element types -------------------------------------------------------------------------------------------
-// Every choice that depends on an element type goes through these helpers, so each of them names all three types.
-__host__ __device__ __forceinline__ bool dtype_valid(int dtype) { return dtype == B2_F32 || dtype == B2_BF16 || dtype == B2_F16; }
-__host__ __device__ constexpr int esize(int dtype) { return dtype == B2_F32 ? 4 : (dtype == B2_BF16 || dtype == B2_F16) ? 2 : 0; }
+// Every choice that depends on an element type goes through these helpers, so each of them names all four types.
+// B2_I8 is read only by the kernels that take a WITH_I8 template flag (and the utility kernels, which always do): the
+// finalize and filter kernels of the floating-point types keep code that never tests for it.
+__host__ __device__ __forceinline__ bool dtype_valid(int dtype) {
+    return dtype == B2_F32 || dtype == B2_BF16 || dtype == B2_F16 || dtype == B2_I8;
+}
+__host__ __device__ constexpr int esize_float(int dtype) { return dtype == B2_F32 ? 4 : (dtype == B2_BF16 || dtype == B2_F16) ? 2 : 0; }
+__host__ __device__ constexpr int esize(int dtype) { return dtype == B2_I8 ? 1 : esize_float(dtype); }
 // elements per 16 bytes: the row pitch of a TMA operand is a multiple of this
 __host__ __device__ constexpr int tma_align_elems(int dtype) { return 16 / esize(dtype); }
+// largest dimension of an int8 index: |<q, x>| <= 2^14 d must stay inside the s32 accumulators of the int8 filter; with L2
+// the filter forms 2 <q, x> - |x|^2 = |q|^2 - |q - x|^2 in int32 too, and |q - x|^2 <= 255^2 d needs d < 2^15
+constexpr int I8_MAX_D = (1 << 17) - 1;
+constexpr int I8_L2_MAX_D = (1 << 15) - 1;
 
 // the fp32 value of the 2-byte pattern `h` (exact for both 2-byte types)
 template <int DT>
@@ -94,7 +103,11 @@ __device__ __forceinline__ float half_bits_f32(uint32_t h) {
 }
 
 // element i of a row-major matrix of `dtype`, as fp32 (exact)
+template <bool WITH_I8 = false>
 __device__ __forceinline__ float elem_f32(const void* base, int dtype, size_t i) {
+    if constexpr (WITH_I8) {
+        if (dtype == B2_I8) return (float)reinterpret_cast<const int8_t*>(base)[i];
+    }
     switch (dtype) {
         case B2_F32: return reinterpret_cast<const float*>(base)[i];
         case B2_BF16: return __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(base)[i]);
@@ -102,11 +115,13 @@ __device__ __forceinline__ float elem_f32(const void* base, int dtype, size_t i)
     }
 }
 
-// out[i] = v rounded to nearest even in `dtype` (|v| >= 65520 becomes inf in fp16)
+// out[i] = v rounded to nearest even in `dtype` (|v| >= 65520 becomes inf in fp16). int8 is written only from values that
+// are int8 already (copies and padding of int8 rows).
 __device__ __forceinline__ void store_elem(void* out, int dtype, size_t i, float v) {
     switch (dtype) {
         case B2_F32: reinterpret_cast<float*>(out)[i] = v; break;
         case B2_BF16: reinterpret_cast<__nv_bfloat16*>(out)[i] = __float2bfloat16_rn(v); break;
+        case B2_I8: reinterpret_cast<int8_t*>(out)[i] = (int8_t)__float2int_rn(v); break;
         default: reinterpret_cast<__half*>(out)[i] = __float2half_rn(v); break;  // B2_F16
     }
 }
@@ -119,6 +134,7 @@ struct MatView {
     const void* store = nullptr;
     const void* filt = nullptr;
     const float* norm2 = nullptr;  // [n] fp32 squared norms of the exact rows (L2 filter epilogue)
+    const int32_t* norm2_i8 = nullptr;  // int8 stores: [n] the same norms as exact integers (int8 L2 filter epilogue)
     int64_t n = 0;
     int32_t d = 0;
     int32_t dtype = B2_F32;       // element type of `store`
@@ -129,6 +145,10 @@ struct MatView {
     // certificate fails there go through the tf32 filter on `filt`.
     const void* filt16 = nullptr;
     int64_t filt16_pitch = 0;
+    // int8 stores only: an fp16 copy of the rows (exact, pitch multiple of 8), built on the first search with fp32 / bf16 / fp16
+    // queries, which cannot use the int8 filter; those searches filter on it with the fp16 wgmma
+    const void* filt_f16 = nullptr;
+    int64_t filt_f16_pitch = 0;
     float max_norm = 0.f;    // max_j ||x_j|| (upper bound), for the certification margin
     const float* max_norm_dev = nullptr;  // when set, the kernels read the bound from device memory instead (no host sync:
                                           // the k-means loop rebuilds its centroid view every iteration)
@@ -154,6 +174,7 @@ int launch_prep_queries(const void* q, int q_dtype, int64_t nq, int d, void* q_f
                         int64_t filt_pitch, cudaStream_t stream);
 int launch_row_norms(const void* x, int dtype, int64_t n, int d, float* norm2, float* max_norm_dev,
                      cudaStream_t stream);
+int launch_row_norms_i8(const void* x, int64_t n, int d, int32_t* norm2, cudaStream_t stream);  // exact, int8 rows
 int launch_convert_pad(const void* x, int dtype, int64_t n, int d, void* out, int out_dtype, int64_t out_pitch,
                        cudaStream_t stream);
 int launch_exact_l2_assigned(const void* pts, int dtype, int64_t m, int d, const float* cent, const int64_t* assign, float* out,

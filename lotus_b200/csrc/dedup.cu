@@ -29,8 +29,8 @@ __global__ void pair_verify_kernel(const char* store, int dtype, int d, const in
         double acc = 0.0;
         for (int g = lane; g < ngroups; g += 32) {
             float a[4], b[4];
-            load_group(ri, dtype, g, d, vec, a);
-            load_group(rj, dtype, g, d, vec, b);
+            load_group<true>(ri, dtype, g, d, vec, a);
+            load_group<true>(rj, dtype, g, d, vec, b);
 #pragma unroll
             for (int e = 0; e < 4; ++e) acc = fma((double)a[e], (double)b[e], acc);
         }

@@ -131,6 +131,7 @@ struct b2_index {
     int32_t dtype = B2_F32;
     int32_t metric = B2_METRIC_IP;
     DevBuf store, filt_pad, filt16, norm2, scalar;
+    DevBuf filt_f16, sub_filt_f16;  // int8 stores: the fp16 copy of the rows (and of an ids subset) for floating-point queries
     MatView view;
     // per-call workspaces
     DevBuf q_in, q_filt, cand_score, cand_id, cand_thr, flags, sel, dense, out_sc, out_id, ids_dev;
@@ -147,6 +148,8 @@ struct b2_index {
         b2::FilterPlan plan;
     } staged;
     DevBuf q_norm2;
+    DevBuf q_wide;  // int8 queries on a floating-point store, widened exactly
+    b2_index* f16_twin = nullptr;  // int8 indexes: the fp16 copy k-means runs on (kmeans_view)
     ~b2_index();  // destroys the stream and events; the buffers free themselves
 };
 
@@ -159,6 +162,8 @@ int build_view(const void* store, int64_t n, int d, int dtype, DevBuf& filt_pad,
 int search_core(b2_index* idx, const MatView& X, int metric, const void* q_dev, int q_dtype, int64_t nq, int k,
                 const int64_t* id_map, int64_t id_offset, float* out_sc, int64_t* out_id, cudaStream_t st, int level = 0);
 float filter_rel_eps(int store_dtype, int filt_dtype, int q_dtype, int d);
+// the index k-means runs on: idx itself, or for an int8 index its fp16 twin (exact), made on first use
+int kmeans_view(b2_index* idx, b2_index** out);
 float filter_abs_eps(int store_dtype, int filt_dtype, int q_dtype, int d);
 // model_sms > 0: plan without a device, modelling the workers as model_sms SMs all in use (b2_debug_filter_plan)
 int plan_filter(const MatView& X, const void* q, int q_dtype, int64_t nq, int k, bool top1, int device, FilterPlan& plan,

@@ -1003,6 +1003,10 @@ extern "C" {
 int b2_kmeans(b2_index* idx, const int64_t* ids, int64_t m, int32_t k, int32_t niter, int64_t seed, int32_t full_lloyd,
               int64_t* out_assign, float* out_centroids, float* out_obj) {
     if (!idx) { set_error("Index not loaded"); return B2_EINVAL; }
+    {
+        DeviceGuard twin_guard(idx->device);
+        B2_TRY(kmeans_view(idx, &idx));
+    }
     if (!ids) m = idx->n;
     if (k <= 0 || niter < 0 || m < 0 || !out_assign) { set_error("bad k-means arguments (k=%d niter=%d m=%lld)", k, niter, (long long)m); return B2_EINVAL; }
     if (m < k) { set_error("Number of training points (%lld) should be at least as large as number of clusters (%d)", (long long)m, k); return B2_EINVAL; }
@@ -1021,6 +1025,10 @@ int b2_kmeans(b2_index* idx, const int64_t* ids, int64_t m, int32_t k, int32_t n
 int b2_kmeans_assign_dev(b2_index* idx, const int64_t* ids_dev, int64_t m, const float* centroids_dev, int32_t k, int64_t* assign_dev,
                          float* dist_dev, void* stream) {
     if (!idx) { set_error("Index not loaded"); return B2_EINVAL; }
+    {
+        DeviceGuard twin_guard(idx->device);
+        B2_TRY(kmeans_view(idx, &idx));
+    }
     if (!ids_dev) m = idx->n;
     if (k <= 0 || m < 0 || !centroids_dev || (m > 0 && !assign_dev)) { set_error("bad arguments"); return B2_EINVAL; }
     if (m == 0) return B2_OK;
@@ -1039,6 +1047,10 @@ int b2_kmeans_assign_dev(b2_index* idx, const int64_t* ids_dev, int64_t m, const
 int b2_kmeans_accumulate_dev(b2_index* idx, const int64_t* ids_dev, int64_t m, const int64_t* assign_dev, int32_t k,
                              const float* centroids_dev, float* sums_dev, float* counts_dev, double* obj_dev, void* stream) {
     if (!idx) { set_error("Index not loaded"); return B2_EINVAL; }
+    {
+        DeviceGuard twin_guard(idx->device);
+        B2_TRY(kmeans_view(idx, &idx));
+    }
     if (!ids_dev) m = idx->n;
     if (k <= 0 || m < 0 || (m > 0 && !assign_dev) || !sums_dev || !counts_dev) { set_error("bad arguments"); return B2_EINVAL; }
     if (obj_dev && !centroids_dev) { set_error("the objective needs the centroids the assignment was made against"); return B2_EINVAL; }
@@ -1055,6 +1067,10 @@ int b2_kmeans_accumulate_dev(b2_index* idx, const int64_t* ids_dev, int64_t m, c
 int b2_kmeans_accumulate(b2_index* idx, const int64_t* ids, int64_t m, const int64_t* assign, int32_t k, float* out_sums,
                          float* out_counts) {
     if (!idx) { set_error("Index not loaded"); return B2_EINVAL; }
+    {
+        DeviceGuard twin_guard(idx->device);
+        B2_TRY(kmeans_view(idx, &idx));
+    }
     if (!ids) m = idx->n;
     if (k <= 0 || m < 0 || !assign || !out_sums || !out_counts) { set_error("bad arguments"); return B2_EINVAL; }
     for (int64_t i = 0; i < m; ++i)
@@ -1087,6 +1103,10 @@ int b2_kmeans_accumulate(b2_index* idx, const int64_t* ids, int64_t m, const int
 int b2_kmeans_assign(b2_index* idx, const int64_t* ids, int64_t m, const float* centroids, int32_t k, int64_t* out_assign,
                      float* out_dist) {
     if (!idx) { set_error("Index not loaded"); return B2_EINVAL; }
+    {
+        DeviceGuard twin_guard(idx->device);
+        B2_TRY(kmeans_view(idx, &idx));
+    }
     if (!ids) m = idx->n;
     if (k <= 0 || m < 0 || !centroids || (m > 0 && !out_assign)) { set_error("bad arguments"); return B2_EINVAL; }
     if (m == 0) return B2_OK;

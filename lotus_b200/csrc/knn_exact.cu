@@ -124,7 +124,7 @@ __global__ void prep_queries_kernel(const void* q, int q_dtype, int64_t nq, int 
     for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
         const int64_t r = t / pitch;
         const int c = (int)(t - r * pitch);
-        const float v = c < d ? elem_f32(q, q_dtype, (size_t)(r * d + c)) : 0.f;
+        const float v = c < d ? elem_f32<true>(q, q_dtype, (size_t)(r * d + c)) : 0.f;
         store_elem(out, out_dtype, (size_t)t, v);
     }
 }
@@ -142,7 +142,7 @@ __global__ void row_norms_kernel(const void* x, int dtype, int64_t n, int d, flo
         const int ngroups = (d + 3) >> 2;
         for (int g = lane; g < ngroups; g += 32) {
             float v[4];
-            load_group(row, dtype, g, d, vec, v);
+            load_group<true>(row, dtype, g, d, vec, v);
 #pragma unroll
             for (int e = 0; e < 4; ++e) acc = fma((double)v[e], (double)v[e], acc);
         }
@@ -153,12 +153,27 @@ __global__ void row_norms_kernel(const void* x, int dtype, int64_t n, int d, flo
     if (lane == 0 && local_max > 0.f) atomicMax(reinterpret_cast<int*>(max_norm), __float_as_int(local_max));
 }
 
+// exact squared norms of int8 rows (<= 2^14 d < 2^31): one warp per row
+__global__ void row_norms_i8_kernel(const int8_t* x, int64_t n, int d, int32_t* norm2) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warp = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
+    const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    for (int64_t j = warp; j < n; j += nwarps) {
+        const int8_t* row = x + (size_t)j * d;
+        int32_t acc = 0;
+        for (int c = lane; c < d; c += 32) acc += (int32_t)row[c] * (int32_t)row[c];
+#pragma unroll
+        for (int off = 16; off >= 1; off >>= 1) acc += __shfl_xor_sync(FULL, acc, off);
+        if (lane == 0) norm2[j] = acc;
+    }
+}
+
 __global__ void convert_pad_kernel(const void* x, int dtype, int64_t n, int d, void* out, int out_dtype, int64_t pitch) {
     const int64_t total = n * pitch;
     for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
         const int64_t r = t / pitch;
         const int c = (int)(t - r * pitch);
-        const float v = c < d ? elem_f32(x, dtype, (size_t)(r * d + c)) : 0.f;
+        const float v = c < d ? elem_f32<true>(x, dtype, (size_t)(r * d + c)) : 0.f;
         store_elem(out, out_dtype, (size_t)t, v);
     }
 }
@@ -181,10 +196,12 @@ __global__ void gather_rows_kernel(const char* x, size_t row_bytes, const int64_
             const int4* s4 = reinterpret_cast<const int4*>(src);
             int4* d4 = reinterpret_cast<int4*>(dst);
             for (size_t t = lane; t < row_bytes / 16; t += 32) d4[t] = __ldg(s4 + t);
-        } else {
+        } else if ((row_bytes & 1) == 0) {
             const uint16_t* s2 = reinterpret_cast<const uint16_t*>(src);
             uint16_t* d2 = reinterpret_cast<uint16_t*>(dst);
             for (size_t t = lane; t < row_bytes / 2; t += 32) d2[t] = s2[t];
+        } else {  // int8 rows of odd d
+            for (size_t t = lane; t < row_bytes; t += 32) dst[t] = src[t];
         }
     }
 }
@@ -199,7 +216,13 @@ __device__ __forceinline__ void canonical_partial_multi(const float* q_s, const 
     const int ngroups = d >> 2;
     for (int g = lane; g < ngroups; g += 32) {
         float x[U][4];
-        if constexpr (DT != B2_F32) {  // B2_BF16, B2_F16
+        if constexpr (DT == B2_I8) {
+            uint32_t t[U];
+#pragma unroll
+            for (int u = 0; u < U; ++u) t[u] = __ldg(reinterpret_cast<const uint32_t*>(rows[u]) + g);
+#pragma unroll
+            for (int u = 0; u < U; ++u) unpack4_i8(t[u], x[u]);
+        } else if constexpr (DT != B2_F32) {  // B2_BF16, B2_F16
             uint2 t[U];
 #pragma unroll
             for (int u = 0; u < U; ++u) t[u] = __ldg(reinterpret_cast<const uint2*>(rows[u]) + g);
@@ -257,8 +280,10 @@ struct FinalizeParams {
 
 constexpr int FIN_WARPS = 4;
 
-template <int R>  // 32*R >= KP candidates survive the merge
-__global__ void __launch_bounds__(FIN_WARPS * 32) finalize_kernel(const FinalizeParams p) {
+// I8: the store is int8 (the queries are of any type). The floating-point stores run the instantiation without it, whose
+// code never tests for int8.
+template <int R, bool I8>
+__device__ __forceinline__ void finalize_body(const FinalizeParams p) {
     constexpr int NC = 32 * R;
     extern __shared__ __align__(16) uint8_t fsm[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -275,10 +300,10 @@ __global__ void __launch_bounds__(FIN_WARPS * 32) finalize_kernel(const Finalize
     const float max_norm = p.max_norm_dev ? __ldg(p.max_norm_dev) : p.max_norm;
     const bool is_l2 = p.metric == B2_METRIC_L2;
     const bool vec = (p.d % 4) == 0;
-    const size_t esz = esize(p.dtype);
+    const size_t esz = I8 ? 1 : esize_float(p.dtype);
 
     // 1. query -> smem (fp32, exact upcast for bf16) and its canonical squared norm
-    for (int i = lane; i < d4; i += 32) q_s[i] = i < p.d ? elem_f32(p.q, p.q_dtype, (size_t)q * p.d + i) : 0.f;
+    for (int i = lane; i < d4; i += 32) q_s[i] = i < p.d ? elem_f32<I8>(p.q, p.q_dtype, (size_t)q * p.d + i) : 0.f;
     __syncwarp();
     double qacc = 0.0;
     for (int g = lane; g < (d4 >> 2); g += 32) {
@@ -380,7 +405,10 @@ __global__ void __launch_bounds__(FIN_WARPS * 32) finalize_kernel(const Finalize
 #pragma unroll
             for (int u = 0; u < 4; ++u)
                 rows[u] = reinterpret_cast<const char*>(p.store) + (size_t)(ids[u] >= 0 ? ids[u] : ids[0]) * p.d * esz;
-            if (p.dtype == B2_BF16) {
+            if constexpr (I8) {
+                if (is_l2) canonical_partial_multi<true, B2_I8, 4>(q_s, rows, p.d, lane, part);
+                else canonical_partial_multi<false, B2_I8, 4>(q_s, rows, p.d, lane, part);
+            } else if (p.dtype == B2_BF16) {
                 if (is_l2) canonical_partial_multi<true, B2_BF16, 4>(q_s, rows, p.d, lane, part);
                 else canonical_partial_multi<false, B2_BF16, 4>(q_s, rows, p.d, lane, part);
             } else if (p.dtype == B2_F16) {
@@ -396,8 +424,8 @@ __global__ void __launch_bounds__(FIN_WARPS * 32) finalize_kernel(const Finalize
                 part[u] = 0.0;
                 if (ids[u] >= 0) {
                     const char* row = reinterpret_cast<const char*>(p.store) + (size_t)ids[u] * p.d * esz;
-                    part[u] = is_l2 ? canonical_partial<true>(q_s, row, p.dtype, p.d, vec, lane)
-                                    : canonical_partial<false>(q_s, row, p.dtype, p.d, vec, lane);
+                    part[u] = is_l2 ? canonical_partial<true, I8>(q_s, row, p.dtype, p.d, vec, lane)
+                                    : canonical_partial<false, I8>(q_s, row, p.dtype, p.d, vec, lane);
                 }
             }
         }
@@ -520,6 +548,11 @@ __global__ void __launch_bounds__(FIN_WARPS * 32) finalize_kernel(const Finalize
     }
 }
 
+template <int R>  // 32*R >= KP candidates survive the merge
+__global__ void __launch_bounds__(FIN_WARPS * 32) finalize_kernel(const FinalizeParams p) { finalize_body<R, false>(p); }
+template <int R>
+__global__ void __launch_bounds__(FIN_WARPS * 32) finalize_i8_kernel(const FinalizeParams p) { finalize_body<R, true>(p); }
+
 // ---- dense exact path -----------------------------------------------------------------------------------------
 // scores[s, j] = canonical score of selected query s against row j. One warp per row; the row's share stays
 // in registers/L1 while the warp walks the selected queries.
@@ -540,14 +573,14 @@ __global__ void dense_scores_kernel(const void* store, int dtype, int64_t n, int
         for (int t = threadIdx.x; t < sc * d4; t += blockDim.x) {
             const int s = t / d4, i = t - s * d4;
             const int64_t qi = q_sel ? q_sel[s0 + s] : (s0 + s);
-            dq[t] = i < d ? elem_f32(q, q_dtype, (size_t)qi * d + i) : 0.f;
+            dq[t] = i < d ? elem_f32<true>(q, q_dtype, (size_t)qi * d + i) : 0.f;
         }
         __syncthreads();
         for (int64_t j = warp; j < n; j += nwarps) {
             const char* row = reinterpret_cast<const char*>(store) + (size_t)j * d * esz;
             for (int s = 0; s < sc; ++s) {
-                const double part = is_l2 ? canonical_partial<true>(dq + s * d4, row, dtype, d, vec, lane)
-                                          : canonical_partial<false>(dq + s * d4, row, dtype, d, vec, lane);
+                const double part = is_l2 ? canonical_partial<true, true>(dq + s * d4, row, dtype, d, vec, lane)
+                                          : canonical_partial<false, true>(dq + s * d4, row, dtype, d, vec, lane);
                 const double tot = butterfly_sum(part);
                 if (lane == 0) out[(size_t)(s0 + s) * n + j] = (float)tot;
             }
@@ -944,6 +977,13 @@ int launch_exact_l2_assigned(const void* pts, int dtype, int64_t m, int d, const
     return B2_OK;
 }
 
+int launch_row_norms_i8(const void* x, int64_t n, int d, int32_t* norm2, cudaStream_t stream) {
+    if (n <= 0) return B2_OK;
+    row_norms_i8_kernel<<<grid_for(n * 32, 256), 256, 0, stream>>>(reinterpret_cast<const int8_t*>(x), n, d, norm2);
+    B2_LAUNCH_CHECK();
+    return B2_OK;
+}
+
 int launch_convert_pad(const void* x, int dtype, int64_t n, int d, void* out, int out_dtype, int64_t out_pitch,
                        cudaStream_t stream) {
     if (n <= 0) return B2_OK;
@@ -966,7 +1006,7 @@ template <int R>
 static int launch_finalize_r(const FinalizeParams& p, cudaStream_t stream) {
     const int d4 = ((p.d + 3) >> 2) << 2;
     const size_t smem = (size_t)FIN_WARPS * ((size_t)d4 * 4 + (size_t)(32 * R) * 16);
-    auto kern = finalize_kernel<R>;
+    auto kern = p.dtype == B2_I8 ? finalize_i8_kernel<R> : finalize_kernel<R>;
     if (smem > 48 * 1024) {
         if (smem > 200 * 1024) {
             set_error("embedding dimension %d too large for the finalize kernel", p.d);

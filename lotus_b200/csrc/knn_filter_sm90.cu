@@ -36,6 +36,9 @@
 // with bit 3 of c equal to e, so a query keeps two lists of KP/2 per corpus split, the layout finalize merges.
 #include <cuda.h>
 
+#include <climits>
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace b2 {
@@ -203,15 +206,17 @@ __device__ __forceinline__ void acc_fence(float (&d)[128]) {
 }
 
 // Operand kind of the filter: the element type both wgmma operands are streamed in. BF16 and F16 are 2-byte operands
-// (m64n256k16, 32 elements per K-block); TF32 reads fp32 operands (m64n256k8, 16 elements per K-block).
-enum class Op { BF16, F16, TF32 };
-__host__ __device__ constexpr int op_bytes(Op op) { return op == Op::TF32 ? 4 : 2; }
+// (m64n256k16, 32 elements per K-block); TF32 reads fp32 operands (m64n256k8, 16 elements per K-block); I8 reads int8
+// operands (m64n256k32 into s32 accumulators, 64 elements per K-block: exact integer products and sums).
+enum class Op { BF16, F16, TF32, I8 };
+__host__ __device__ constexpr int op_bytes(Op op) { return op == Op::TF32 ? 4 : op == Op::I8 ? 1 : 2; }
 
 // the 128 accumulators of an m64n256 wgmma, as operands %0..%127
 #define B2_WGMMA_D                                                                                                           \
     "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}"
 #define B2_WGMMA_D_OPS                                                                                                       \
     "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+#define B2_WGMMA_D_OPS_S32 "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]), "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]), "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63]), "+r"(d[64]), "+r"(d[65]), "+r"(d[66]), "+r"(d[67]), "+r"(d[68]), "+r"(d[69]), "+r"(d[70]), "+r"(d[71]), "+r"(d[72]), "+r"(d[73]), "+r"(d[74]), "+r"(d[75]), "+r"(d[76]), "+r"(d[77]), "+r"(d[78]), "+r"(d[79]), "+r"(d[80]), "+r"(d[81]), "+r"(d[82]), "+r"(d[83]), "+r"(d[84]), "+r"(d[85]), "+r"(d[86]), "+r"(d[87]), "+r"(d[88]), "+r"(d[89]), "+r"(d[90]), "+r"(d[91]), "+r"(d[92]), "+r"(d[93]), "+r"(d[94]), "+r"(d[95]), "+r"(d[96]), "+r"(d[97]), "+r"(d[98]), "+r"(d[99]), "+r"(d[100]), "+r"(d[101]), "+r"(d[102]), "+r"(d[103]), "+r"(d[104]), "+r"(d[105]), "+r"(d[106]), "+r"(d[107]), "+r"(d[108]), "+r"(d[109]), "+r"(d[110]), "+r"(d[111]), "+r"(d[112]), "+r"(d[113]), "+r"(d[114]), "+r"(d[115]), "+r"(d[116]), "+r"(d[117]), "+r"(d[118]), "+r"(d[119]), "+r"(d[120]), "+r"(d[121]), "+r"(d[122]), "+r"(d[123]), "+r"(d[124]), "+r"(d[125]), "+r"(d[126]), "+r"(d[127])
 #define B2_WGMMA_64X256(SHAPE_TYPES, IMM_TAIL)                                                                               \
     asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"                                                   \
                  "wgmma.mma_async.sync.aligned." SHAPE_TYPES " " B2_WGMMA_D ", %128, %129, p, 1, 1" IMM_TAIL ";\n\t}"         \
@@ -247,8 +252,32 @@ __device__ __forceinline__ void wgmma_64x256_rs(float (&d)[128], const uint32_t*
         B2_WGMMA_64X256_RS("m64n256k16.f32.bf16.bf16", ", 0");
     }
 }
+// The int8 product into s32 accumulators: integer wgmma takes neither scale nor transpose immediates.
+template <Op OP>
+__device__ __forceinline__ void wgmma_64x256(int32_t (&d)[128], uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
+    static_assert(OP == Op::I8, "s32 accumulators take int8 operands");
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n256k32.s32.s8.s8 " B2_WGMMA_D ", %128, %129, p;\n\t}"
+                 : B2_WGMMA_D_OPS_S32
+                 : "l"(adesc), "l"(bdesc), "r"(scale_d));
+}
+// register A: a k32 step of int8 has the byte layout of a k16 step of a 2-byte type (register j: row (lane / 4) + 8 (j & 1),
+// bytes 4 (lane % 4) + 16 (j >> 1) .. + 3 of the step's 32), so load_a_frag's ldmatrix path fills it unchanged
+template <Op OP>
+__device__ __forceinline__ void wgmma_64x256_rs(int32_t (&d)[128], const uint32_t* a, uint64_t bdesc, uint32_t scale_d) {
+    static_assert(OP == Op::I8, "s32 accumulators take int8 operands");
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %133, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n256k32.s32.s8.s8 " B2_WGMMA_D ", {%128, %129, %130, %131}, %132, p;\n\t}"
+                 : B2_WGMMA_D_OPS_S32
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(scale_d));
+}
+__device__ __forceinline__ void acc_fence(int32_t (&d)[128]) {
+#pragma unroll
+    for (int i = 0; i < 128; ++i) asm volatile("" : "+r"(d[i])::"memory");
+}
 #undef B2_WGMMA_64X256_RS
 #undef B2_WGMMA_64X256
+#undef B2_WGMMA_D_OPS_S32
 #undef B2_WGMMA_D_OPS
 #undef B2_WGMMA_D
 
@@ -313,6 +342,7 @@ struct FilterParams {
     int32_t* pair_j;
     unsigned long long* pair_count;   // total candidates found (may exceed pair_cap)
     unsigned long long pair_cap;
+    const int32_t* xnorm_i;  // [n] exact squared norms of int8 rows (int8 L2 filter epilogue)
 };
 
 struct Ring {
@@ -442,8 +472,8 @@ __device__ __forceinline__ void release_stage(const Ring& r, int s, int cta) {
 // K-blocks kb < RES_KB take A from `afrag`, which holds them for the whole item: the item's first tile (load_a) fills it from
 // the landed stages, later tiles find no A in those stages (producer_loop). The rest read A from shared memory. The operands
 // and the K order are the same either way, so are the accumulators.
-template <Op OP, int NSTAGES, int CL, int RES_KB>
-__device__ __forceinline__ void mma_tile(float (&acc)[128], uint32_t (&afrag)[RES_KB > 0 ? RES_KB : 1][KB_AREGS], bool load_a,
+template <Op OP, int NSTAGES, int CL, int RES_KB, typename AccT>
+__device__ __forceinline__ void mma_tile(AccT (&acc)[128], uint32_t (&afrag)[RES_KB > 0 ? RES_KB : 1][KB_AREGS], bool load_a,
                                          const Ring& r, int num_kb, int g, int cta, int& stage, uint32_t& phase) {
     const uint32_t a_off = (uint32_t)(g * WG_M * KB_BYTES);
     int prev = -1;
@@ -636,10 +666,20 @@ __device__ __forceinline__ void process8_top2(const float (&v)[8], int idx0, flo
     }
 }
 
-template <int KP, bool IS_L2, Op OP, int CL, bool TOP1 = false>
-__global__ void __launch_bounds__(NUM_THREADS, 1)
-knn_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_x,
-                  const FilterParams p) {
+// The knn filter. Op::I8 accumulates in s32 and runs its gate on integers: the score s (IP) or 2 s - |x|^2 (L2, exact in int32
+// for d < 2^15 since it equals |q|^2 - |q - x|^2) against the list thresholds rounded down. Only the chunks that pass are
+// converted to fp32 (once, round to nearest), before the transpose, so the lists keep their fp32 format.
+// int8 filter score of accumulator s for corpus column j: s (IP) or 2 s - |x_j|^2 (L2), exact in int32 (unsigned arithmetic:
+// the intermediate 2 s may wrap, the result does not); `valid` is false past the corpus end, where the row norm is not read
+template <bool IS_L2>
+__device__ __forceinline__ int32_t i8_score(int32_t s, const FilterParams& p, int j, bool valid) {
+    if constexpr (IS_L2) return valid ? (int32_t)(2u * (uint32_t)s - (uint32_t)__ldg(p.xnorm_i + j)) : s;
+    else return s;
+}
+
+template <int KP, bool IS_L2, Op OP, int CL, bool TOP1>
+__device__ __forceinline__ void knn_filter_body(const CUtensorMap& tmap_q, const CUtensorMap& tmap_x, const FilterParams& p) {
+    using AccT = std::conditional_t<OP == Op::I8, int32_t, float>;
     constexpr int NSTAGES = num_stages(KP);
     static_assert(NSTAGES >= 2, "not enough shared memory for the operand ring");
     constexpr int KPH = KP / 2;  // candidates kept per (row, set)
@@ -679,7 +719,7 @@ knn_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
         const int fr = lane >> 2, fc = 2 * (lane & 3);
         int stage = 0;
         uint32_t phase = 0;
-        float acc[128];
+        AccT acc[128];
         uint32_t afrag[RES_KB][KB_AREGS];  // the query tile's first RES_KB K-blocks, loaded in each item's first tile
         for (int item = sc.worker; item < n_items; item += sc.n_workers) {
             int m_tile, split, t0, t1;
@@ -699,6 +739,8 @@ knn_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
             // thresholds of the lists this lane's fragment values go to: gthr[h][s] is (row fr + 8h, set s), the `thr` of
             // lane fr + 8h + 16s
             float gthr[2][2] = {{-INFINITY, -INFINITY}, {-INFINITY, -INFINITY}};
+            // int8: gthr rounded down (an integer score s beats t exactly when s > floor(t); -inf maps to INT_MIN)
+            int32_t gthr_i[2][2] = {{INT_MIN, INT_MIN}, {INT_MIN, INT_MIN}};
             for (int t = t0; t < t1; ++t) {
                 mma_tile<OP, NSTAGES, CL, RES_KB>(acc, afrag, t == t0, ring, p.num_kb, g, sc.cta, stage, phase);
                 const int col0 = t * BLOCK_N;
@@ -715,11 +757,16 @@ knn_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
 #pragma unroll
                             for (int h = 0; h < 4; ++h) {  // acc[a + h]: row fr + 8 (h >> 1), column 16c + 8jj + fc + (h & 1)
                                 const int off = 16 * c + 8 * jj + fc + (h & 1);
-                                float s = acc[(2 * c + jj) * 4 + h];
-                                if constexpr (IS_L2) {
-                                    if (off < ncols) s = fmaf(2.f, s, -__ldg(p.xnorm + col0 + off));
+                                if constexpr (OP == Op::I8) {
+                                    hit |= off < ncols && i8_score<IS_L2>(acc[(2 * c + jj) * 4 + h], p, col0 + off, off < ncols) >
+                                                              gthr_i[h >> 1][jj];
+                                } else {
+                                    float s = (float)acc[(2 * c + jj) * 4 + h];
+                                    if constexpr (IS_L2) {
+                                        if (off < ncols) s = fmaf(2.f, s, -__ldg(p.xnorm + col0 + off));
+                                    }
+                                    hit |= off < ncols && s > gthr[h >> 1][jj];
                                 }
-                                hit |= off < ncols && s > gthr[h >> 1][jj];
                             }
                         }
                         if (!__any_sync(0xffffffffu, hit)) continue;
@@ -728,17 +775,25 @@ knn_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
 #pragma unroll
                     for (int jj = 0; jj < 2; ++jj) {
                         const int a = (2 * c + jj) * 4;
-                        xs[fr * XP_STRIDE + 8 * jj + fc] = acc[a];
-                        xs[fr * XP_STRIDE + 8 * jj + fc + 1] = acc[a + 1];
-                        xs[(fr + 8) * XP_STRIDE + 8 * jj + fc] = acc[a + 2];
-                        xs[(fr + 8) * XP_STRIDE + 8 * jj + fc + 1] = acc[a + 3];
+                        if constexpr (OP == Op::I8) {  // the gate's integer scores, rounded to nearest: the only error
+                            const int off = 16 * c + 8 * jj + fc;
+                            xs[fr * XP_STRIDE + 8 * jj + fc] = (float)i8_score<IS_L2>(acc[a], p, col0 + off, off < ncols);
+                            xs[fr * XP_STRIDE + 8 * jj + fc + 1] = (float)i8_score<IS_L2>(acc[a + 1], p, col0 + off + 1, off + 1 < ncols);
+                            xs[(fr + 8) * XP_STRIDE + 8 * jj + fc] = (float)i8_score<IS_L2>(acc[a + 2], p, col0 + off, off < ncols);
+                            xs[(fr + 8) * XP_STRIDE + 8 * jj + fc + 1] = (float)i8_score<IS_L2>(acc[a + 3], p, col0 + off + 1, off + 1 < ncols);
+                        } else {
+                            xs[fr * XP_STRIDE + 8 * jj + fc] = acc[a];
+                            xs[fr * XP_STRIDE + 8 * jj + fc + 1] = acc[a + 1];
+                            xs[(fr + 8) * XP_STRIDE + 8 * jj + fc] = acc[a + 2];
+                            xs[(fr + 8) * XP_STRIDE + 8 * jj + fc + 1] = acc[a + 3];
+                        }
                     }
                     __syncwarp();
                     float v[8];
 #pragma unroll
                     for (int j = 0; j < 8; ++j) v[j] = xs[rr * XP_STRIDE + 8 * e + j];
                     const int off = 16 * c + 8 * e;
-                    prepare8<IS_L2>(v, col0 + off, ncols - off, p.xnorm);
+                    prepare8<IS_L2 && OP != Op::I8>(v, col0 + off, ncols - off, p.xnorm);  // int8: transformed already
                     if constexpr (TOP1) {
                         process8_top2(v, col0 + off, b1, b2, b3, i1, i2);
                     } else {
@@ -748,6 +803,13 @@ knn_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
                         for (int h = 0; h < 2; ++h) {
 #pragma unroll
                             for (int s = 0; s < 2; ++s) gthr[h][s] = __shfl_sync(0xffffffffu, thr, fr + 8 * h + 16 * s);
+                        }
+                        if constexpr (OP == Op::I8) {
+#pragma unroll
+                            for (int h = 0; h < 2; ++h) {
+#pragma unroll
+                                for (int s = 0; s < 2; ++s) gthr_i[h][s] = __float2int_rd(gthr[h][s]);
+                            }
                         }
                     }
                 }
@@ -791,13 +853,29 @@ knn_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
     teardown_ring<CL>();
 }
 
+template <int KP, bool IS_L2, Op OP, int CL, bool TOP1 = false>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+knn_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_x,
+                  const FilterParams p) {
+    knn_filter_body<KP, IS_L2, OP, CL, TOP1>(tmap_q, tmap_x, p);
+}
+
+// the int8 knn filter (IGMMA): an entry of its own, apart from the floating-point kernels (HGMMA)
+template <int KP, bool IS_L2, int CL>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+knn_i8_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_x,
+                     const FilterParams p) {
+    knn_filter_body<KP, IS_L2, Op::I8, CL, false>(tmap_q, tmap_x, p);
+}
+
 // ---- all-pairs threshold filter (sem_dedup): same mainloop, the epilogue emits (i, j) candidates -------------------
 constexpr int PAIR_STAGES = MAX_STAGES;
 constexpr int PAIR_SMEM = PAIR_STAGES * STAGE_BYTES + BAR_BYTES + SMEM_ALIGN_SLACK;
 
+// Op::I8 compares the s32 scores against the threshold rounded down (s > thr exactly when s > floor(thr))
 template <Op OP, int CL>
-__global__ void __launch_bounds__(NUM_THREADS, 1)
-pair_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_x, const FilterParams p) {
+__device__ __forceinline__ void pair_filter_body(const CUtensorMap& tmap_q, const CUtensorMap& tmap_x, const FilterParams p) {
+    using AccT = std::conditional_t<OP == Op::I8, int32_t, float>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = align_smem(smem_raw);
     const int warp = threadIdx.x >> 5;
@@ -812,10 +890,12 @@ pair_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_cons
         setmaxnreg_inc<232>();
         const int g = (warp >> 2) - 1;
         const int wq = warp & 3;
-        const float thr = p.pair_thr;
+        AccT thr;
+        if constexpr (OP == Op::I8) thr = __float2int_rd(p.pair_thr);
+        else thr = p.pair_thr;
         int stage = 0;
         uint32_t phase = 0;
-        float acc[128];
+        AccT acc[128];
         uint32_t no_afrag[1][KB_AREGS];  // every K-block reads A from shared memory
         for (int item = sc.worker; item < n_items; item += sc.n_workers) {
             int m_tile, split, t0, t1;
@@ -824,9 +904,12 @@ pair_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_cons
             for (int t = t0; t < t1; ++t) {
                 mma_tile<OP, PAIR_STAGES, CL, 0>(acc, no_afrag, false, ring, p.num_kb, g, sc.cta, stage, phase);
                 const int col0 = t * BLOCK_N + 2 * (lane & 3);
-                float mx = acc[0];
+                AccT mx = acc[0];
 #pragma unroll
-                for (int i = 1; i < 128; ++i) mx = fmaxf(mx, acc[i]);
+                for (int i = 1; i < 128; ++i) {
+                    if constexpr (OP == Op::I8) mx = max(mx, acc[i]);
+                    else mx = fmaxf(mx, acc[i]);
+                }
                 if (mx > thr && gi0 < p.n) {
 #pragma unroll
                     for (int i = 0; i < 128; ++i) {
@@ -845,6 +928,19 @@ pair_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_cons
         }
     }
     teardown_ring<CL>();
+}
+
+template <Op OP, int CL>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+pair_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_x, const FilterParams p) {
+    pair_filter_body<OP, CL>(tmap_q, tmap_x, p);
+}
+
+// the int8 all-pairs filter (IGMMA), an entry of its own like knn_i8_filter_kernel
+template <int CL>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+pair_i8_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_x, const FilterParams p) {
+    pair_filter_body<Op::I8, CL>(tmap_q, tmap_x, p);
 }
 
 // ---- host side ---------------------------------------------------------------------------------------------
@@ -871,6 +967,7 @@ Op filter_op(int filt_dtype) {
     switch (filt_dtype) {
         case B2_F32: return Op::TF32;
         case B2_BF16: return Op::BF16;
+        case B2_I8: return Op::I8;
         default: return Op::F16;  // B2_F16
     }
 }
@@ -878,6 +975,7 @@ CUtensorMapDataType tma_data_type(Op op) {
     switch (op) {
         case Op::TF32: return CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
         case Op::BF16: return CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+        case Op::I8: return CU_TENSOR_MAP_DATA_TYPE_UINT8;  // raw bytes, no conversion
         default: return CU_TENSOR_MAP_DATA_TYPE_FLOAT16;  // Op::F16
     }
 }
@@ -940,6 +1038,13 @@ int launch_op(Op op, const CUtensorMap& tq, const CUtensorMap& tx, const FilterP
     switch (op) {
         case Op::TF32: return launch_variant<KP, IS_L2, Op::TF32, CL, TOP1>(tq, tx, p, grid, stream);
         case Op::BF16: return launch_variant<KP, IS_L2, Op::BF16, CL, TOP1>(tq, tx, p, grid, stream);
+        case Op::I8:
+            if constexpr (TOP1) {
+                set_error("internal: no int8 top-1 filter (k-means does not take int8 points)");
+                return B2_EINVAL;
+            } else {
+                return launch_cluster(knn_i8_filter_kernel<KP, IS_L2, CL>, grid, smem_bytes(KP), CL, tq, tx, p, stream);
+            }
         default: return launch_variant<KP, IS_L2, Op::F16, CL, TOP1>(tq, tx, p, grid, stream);  // Op::F16
     }
 }
@@ -1140,6 +1245,7 @@ int launch_knn_filter(const MatView& X, const void* q_filt, int64_t q_pitch, int
     B2_TRY(make_tmap(&tx, X.filt, op, X.n, op_cols, X.filt_pitch, BLOCK_N / cluster));
     FilterParams p;
     p.xnorm = X.norm2;
+    p.xnorm_i = X.norm2_i8;
     p.cand_score = cand_score;
     p.cand_id = cand_id;
     p.cand_thr = cand_thr;
@@ -1184,7 +1290,7 @@ int launch_knn_filter(const MatView& X, const void* q_filt, int64_t q_pitch, int
         B2_TRY(launch_fill_f32(cand_thr, nq * (int64_t)n_splits * 2, -INFINITY, stream));
     }
     const bool is_l2 = metric == B2_METRIC_L2;
-    if (is_l2 && !X.norm2) {
+    if (is_l2 && (!X.norm2 || (op == Op::I8 && !X.norm2_i8))) {
         set_error("internal: L2 filter without row norms");
         return B2_EINVAL;
     }
@@ -1266,6 +1372,9 @@ int launch_pair_filter(const MatView& X, float thr, int part, int nparts, int32_
         case Op::BF16:
             return two_cta ? launch_cluster(pair_filter_kernel<Op::BF16, 2>, grid, PAIR_SMEM, 2, tq, tx, p, stream)
                            : launch_cluster(pair_filter_kernel<Op::BF16, 1>, grid, PAIR_SMEM, 1, tq, tx, p, stream);
+        case Op::I8:
+            return two_cta ? launch_cluster(pair_i8_filter_kernel<2>, grid, PAIR_SMEM, 2, tq, tx, p, stream)
+                           : launch_cluster(pair_i8_filter_kernel<1>, grid, PAIR_SMEM, 1, tq, tx, p, stream);
         default:  // Op::F16
             return two_cta ? launch_cluster(pair_filter_kernel<Op::F16, 2>, grid, PAIR_SMEM, 2, tq, tx, p, stream)
                            : launch_cluster(pair_filter_kernel<Op::F16, 1>, grid, PAIR_SMEM, 1, tq, tx, p, stream);

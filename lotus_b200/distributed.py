@@ -24,16 +24,16 @@ def shard_bounds(n: int, world: int, rank: int) -> tuple[int, int]:
 
 
 def torch_dtype_code(t) -> int:
-    """Native element type code of a torch tensor of float32, bfloat16 or float16; TypeError for anything else."""
+    """Native element type code of a torch tensor of float32, bfloat16, float16 or int8; TypeError for anything else."""
     import torch
-    codes = {torch.float32: nv.F32, torch.bfloat16: nv.BF16, torch.float16: nv.F16}
+    codes = {torch.float32: nv.F32, torch.bfloat16: nv.BF16, torch.float16: nv.F16, torch.int8: nv.I8}
     if t.dtype not in codes:
-        raise TypeError(f"tensor must be float32, bfloat16 or float16, got {t.dtype}")
+        raise TypeError(f"tensor must be float32, bfloat16, float16 or int8, got {t.dtype}")
     return codes[t.dtype]
 
 
 class ShardedIndex:
-    """Each rank holds `local_rows` (a torch CUDA tensor [n_local, d], bf16, fp16 or fp32) = its slice of the corpus."""
+    """Each rank holds `local_rows` (a torch CUDA tensor [n_local, d], bf16, fp16, fp32 or int8) = its slice of the corpus."""
 
     def __init__(self, local_rows, row_offset: int, metric: int = nv.METRIC_IP, group=None):
         import torch

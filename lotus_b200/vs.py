@@ -89,18 +89,48 @@ def f32_to_f16_checked(f: np.ndarray) -> np.ndarray:
     return h
 
 
+def _as_int8(a: Any) -> np.ndarray:
+    """The int8 matrix holding exactly the values of `a` (numpy or torch, any numeric type): every value must be an integer in
+    [-128, 127], otherwise ValueError. The store never picks a quantization scale."""
+    try:
+        import torch
+        if isinstance(a, torch.Tensor):
+            a = a.detach().cpu().numpy() if a.dtype != torch.bfloat16 else a.detach().to(torch.float32).cpu().numpy()
+    except ImportError:  # pragma: no cover
+        pass
+    arr = np.asarray(a)
+    if arr.ndim != 2:
+        raise ValueError(f"embeddings must be 2-D, got shape {arr.shape}")
+    if arr.dtype == np.int8:
+        return np.ascontiguousarray(arr)
+    if arr.dtype.kind not in "iuf" or arr.dtype.kind == "f" and not np.isfinite(arr).all():
+        raise ValueError(f"dtype='i8' needs integer values in [-128, 127]; got {arr.dtype} data")
+    if arr.size and (arr.min() < -128 or arr.max() > 127 or (arr.dtype.kind == "f" and not (arr == np.round(arr)).all())):
+        raise ValueError("dtype='i8' needs integer values in [-128, 127] (quantize the embeddings first; the store never "
+                         "picks a scale)")
+    return np.ascontiguousarray(arr, dtype=np.int8)
+
+
 def _to_host_matrix(a: Any, want_bf16: bool, exact_bf16_ok: bool = False, scratch: "dict | None" = None,
-                    want_f16: bool = False, pass_f16: bool = False):
+                    want_f16: bool = False, pass_f16: bool = False, want_i8: bool = False, pass_i8: bool = False):
     """-> (array for the C-ABI, native dtype code, float32 view of the stored values).
     exact_bf16_ok: when every float32 value is bfloat16-representable (e.g. vectors fetched from a bf16 index,
     sem_sim_join.py:112-118 -> :130-134) ship the exact 2-byte patterns instead: half the H2D bytes and the exact-operand
     error bound in the certificate. Decided from the values themselves on every call (one threaded host pass).
     want_f16: store as float16 (float16 input as it is, anything else rounded once; overflow raises ValueError).
-    pass_f16: float16 input (numpy or torch) is shipped as it is, as 2-byte F16 operands (queries: exact in fp32)."""
+    pass_f16: float16 input (numpy or torch) is shipped as it is, as 2-byte F16 operands (queries: exact in fp32).
+    want_i8: store as int8 (integer values in [-128, 127] only, see _as_int8).
+    pass_i8: int8 input (numpy or torch) is shipped as it is, as 1-byte I8 operands (queries: exact on every store)."""
+    if want_i8:
+        x = _as_int8(a)
+        return x, nv.I8, x.astype(np.float32)
     try:
         import torch
         if isinstance(a, torch.Tensor):
             t = a.detach()
+            if t.dtype == torch.int8 and pass_i8:
+                x = np.ascontiguousarray(t.cpu().numpy())
+                return x, nv.I8, x.astype(np.float32)
             if t.dtype == torch.float16 and (want_f16 or pass_f16) and not want_bf16:
                 a = t.contiguous().cpu().numpy()  # float16 ndarray: handled below
             elif t.dtype == torch.bfloat16 or want_bf16:
@@ -111,6 +141,11 @@ def _to_host_matrix(a: Any, want_bf16: bool, exact_bf16_ok: bool = False, scratc
     except ImportError:  # pragma: no cover
         pass
     arr = np.asarray(a)
+    if arr.dtype == np.int8 and pass_i8:
+        if arr.ndim != 2:
+            raise ValueError(f"embeddings must be 2-D, got shape {arr.shape}")
+        x = np.ascontiguousarray(arr)
+        return x, nv.I8, x.astype(np.float32)
     if arr.dtype == np.float16 and (want_f16 or pass_f16) and not want_bf16:
         if arr.ndim != 2:
             raise ValueError(f"embeddings must be 2-D, got shape {arr.shape}")
@@ -225,7 +260,11 @@ class B200VS(VS):
     dtype: "f32" (store what faiss would: float32), "bf16" (round the corpus to bfloat16 once; exact search
     over those values), "f16" (store float16: float16 embeddings as they are, anything else rounded once, and a value
     outside float16's range raises ValueError; searched at the bf16 rate with results equal to faiss on the float32
-    upcast of the stored values), or "auto" (bf16 only when handed a bf16 tensor, float32 otherwise).
+    upcast of the stored values), "i8" (store int8: embeddings whose values are all integers in [-128, 127], such as
+    quantized embeddings, of any numeric type; anything else raises ValueError, as the store never picks a scale. int8 queries
+    are searched on the int8 tensor cores, floating-point queries against an fp16 copy of the rows made on their first
+    search; results equal faiss on the float32 upcast; dedup and k-means are not available), or "auto" (bf16 only when
+    handed a bf16 tensor, float32 otherwise; int8 input still gives a float32 store).
     """
 
     accepts_id_arrays = True  # `ids=` may be a numpy int64 array (the operators then skip building a Python list)
@@ -237,8 +276,8 @@ class B200VS(VS):
             raise ValueError(f"B200VS implements the flat (exact) index only; factory_string={factory_string!r}")
         if metric not in (METRIC_INNER_PRODUCT, METRIC_L2):
             raise ValueError("metric must be METRIC_INNER_PRODUCT (0) or METRIC_L2 (1)")
-        if dtype not in ("auto", "f32", "bf16", "f16"):
-            raise ValueError("dtype must be 'auto', 'f32', 'bf16' or 'f16'")
+        if dtype not in ("auto", "f32", "bf16", "f16", "i8"):
+            raise ValueError("dtype must be 'auto', 'f32', 'bf16', 'f16' or 'i8'")
         self.factory_string = factory_string
         self.metric = metric
         self.dtype = dtype
@@ -260,12 +299,21 @@ class B200VS(VS):
             if t is not None:
                 import torch
                 want16 = want16 or (self.dtype == "auto" and t.dtype == torch.bfloat16)
-            host, code, _ = _to_host_matrix(embeddings, want16, want_f16=self.dtype == "f16")
+            host, code, _ = _to_host_matrix(embeddings, want16, want_f16=self.dtype == "f16", want_i8=self.dtype == "i8")
             return MultiDeviceIndex(host, code, self.metric, self.devices)  # type: ignore[return-value]
         if t is not None and t.dim() == 2 and t.device.index == self.device:
             # device hand-off: the encoder's output never visits the host on its way into the index (a tensor that
             # already has the store's type is read in place)
             import torch
+            if self.dtype == "i8":
+                src = t.detach()
+                if src.dtype != torch.int8:
+                    fl = src.to(torch.float32)
+                    if not bool(((fl == fl.round()) & (fl >= -128) & (fl <= 127)).all()):
+                        raise ValueError("dtype='i8' needs integer values in [-128, 127] (quantize the embeddings first; the "
+                                         "store never picks a scale)")
+                t = src.to(torch.int8).contiguous()
+                return nv.Index(None, nv.I8, self.metric, self.device, on_device_ptr=t.data_ptr(), n=t.shape[0], d=t.shape[1])
             if self.dtype == "f16":
                 want = torch.float16
             else:
@@ -276,7 +324,8 @@ class B200VS(VS):
                 raise ValueError("embeddings hold values outside the float16 range (|v| < 65520); use dtype='f32' or 'bf16'")
             code = {torch.float32: nv.F32, torch.bfloat16: nv.BF16, torch.float16: nv.F16}[want]
             return nv.Index(None, code, self.metric, self.device, on_device_ptr=t.data_ptr(), n=t.shape[0], d=t.shape[1])
-        host, code, _ = _to_host_matrix(embeddings, self.dtype == "bf16", want_f16=self.dtype == "f16")
+        host, code, _ = _to_host_matrix(embeddings, self.dtype == "bf16", want_f16=self.dtype == "f16",
+                                        want_i8=self.dtype == "i8")
         return nv.Index(host, code, self.metric, self.device)
 
     def _remember(self, index_dir: str, idx: nv.Index, vecs: Any) -> None:
@@ -349,7 +398,7 @@ class B200VS(VS):
         out = idx.gather(ids_a)
         if idx.dtype == nv.BF16:
             return BF16Backed.wrap(nv.bf16_bits_to_f32(out))
-        return out  # float32, or the float16 values of an fp16 index (like pickle.load(vecs)[ids] of float16 vecs)
+        return out  # float32, or the float16 / int8 values of an fp16 / int8 index (like pickle.load(vecs)[ids])
 
     def __call__(self, query_vectors: Any, K: int, ids: list[int] | None = None, **kwargs: Any) -> RMOutput:
         """faiss_vs.py:43-77. Returns float32 distances [Q,K] and int64 indices [Q,K] (global ids; -1 = no result).
@@ -361,7 +410,7 @@ class B200VS(VS):
         if t is not None and ids_a is None and t.dim() == 2 and t.device.index == self.device and not isinstance(self.b2_index, MultiDeviceIndex):
             return self._call_device(t, int(K))
         q, code, _ = _to_host_matrix(query_vectors, False, exact_bf16_ok=self.b2_index.dtype == nv.BF16, scratch=self._scratch,
-                                     pass_f16=True)
+                                     pass_f16=True, pass_i8=True)
         if q.shape[1] != self.b2_index.d:
             raise ValueError(f"query dimension {q.shape[1]} does not match the index dimension {self.b2_index.d}")
         try:
@@ -379,8 +428,8 @@ class B200VS(VS):
         if t.shape[1] != self.b2_index.d:
             raise ValueError(f"query dimension {t.shape[1]} does not match the index dimension {self.b2_index.d}")
         q = t.detach()
-        q = q.contiguous() if q.dtype in (torch.float32, torch.bfloat16, torch.float16) else q.to(torch.float32).contiguous()
-        code = {torch.float32: nv.F32, torch.bfloat16: nv.BF16, torch.float16: nv.F16}[q.dtype]
+        q = q.contiguous() if q.dtype in (torch.float32, torch.bfloat16, torch.float16, torch.int8) else q.to(torch.float32).contiguous()
+        code = {torch.float32: nv.F32, torch.bfloat16: nv.BF16, torch.float16: nv.F16, torch.int8: nv.I8}[q.dtype]
         out_s = torch.empty((q.shape[0], K), dtype=torch.float32, device=q.device)
         out_i = torch.empty((q.shape[0], K), dtype=torch.int64, device=q.device)
         try:
