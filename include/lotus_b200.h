@@ -98,6 +98,22 @@ B2_API int b2_max_k(void);
  * The matrix is copied; the caller may free x afterwards. */
 B2_API int b2_index_create(const void* x, int64_t n, int32_t d, int32_t dtype, int32_t metric, int32_t device,
                     int32_t x_on_device, b2_index** out);
+/* Build a HOST-RESIDENT flat index over the host matrix x[n,d]: for corpora larger than free device memory. The rows are
+ * copied into a library-owned pinned, mapped host allocation (B2_ENOMEM, with the size in the message, when it cannot be
+ * pinned); only their norms (4 bytes per row, 8 for B2_I8), a ring of two chunk slots of ring_bytes in all (0 = 1 GiB) and
+ * per-search workspaces live on the device. fp32 indexes of at least 4096 rows also keep a bf16 rounding of the rows in
+ * pinned memory (2 more bytes per element): the first level of a search streams it. A search streams the rows through the
+ * ring in chunks (rows per chunk from ring_bytes, a multiple of 256), copying the next chunk while the filter runs over the
+ * current one, and returns results bit-identical to b2_index_create's index over the same rows. n < 2^31; every dtype with
+ * the limits of b2_index_create. b2_index_search / _search_dev (with or without ids), b2_index_gather, b2_last_filter_ms (the
+ * sum over chunks) and b2_debug_filter_lists (the folded lists) serve it; b2_index_data_dev returns NULL, and
+ * b2_threshold_pairs, the k-means entry points and b2_index_search_packed_dev / _stage1_dev / _stage2_packed_dev return
+ * B2_EINVAL ("not available on a host-resident index"). An ids subset whose rows fit in the ring is gathered into device
+ * memory and searched there; a larger one is gathered on the host and streamed. */
+B2_API int b2_index_create_host(const void* x, int64_t n, int32_t d, int32_t dtype, int32_t metric, int32_t device,
+                                int64_t ring_bytes, b2_index** out);
+/* where the rows of an index live: 0 = device memory (b2_index_create), 1 = host memory (b2_index_create_host) */
+B2_API int32_t b2_index_resident(const b2_index* idx);
 B2_API void b2_index_free(b2_index* idx);
 B2_API int64_t b2_index_ntotal(const b2_index* idx);
 B2_API int32_t b2_index_dim(const b2_index* idx);
@@ -218,6 +234,17 @@ B2_API int b2_debug_filter_plan(int64_t nq, int64_t n, int32_t k, int32_t num_sm
  * chunk. For testing; not part of the search path. */
 B2_API int b2_debug_filter_lists(b2_index* idx, const void* q, int64_t nq, int32_t q_dtype, int32_t k, int32_t top1, int32_t level,
                           int32_t* plan, float* rel_eps, float* cand_score, int32_t* cand_id, float* cand_thr);
+/* The chunking of a host-resident index of n rows (no device work): *chunk_rows rows per chunk (a multiple of 256 unless
+ * one chunk holds every row), *n_chunks chunks, *slots device slots of the ring. Chunk c owns the rows
+ * [c * chunk_rows, min(n, (c + 1) * chunk_rows)); it streams chunk_rows rows from min(c * chunk_rows, n - chunk_rows) on,
+ * so the last chunk re-streams the tail of its predecessor and the search skips those rows there. B2_EINVAL when a slot
+ * of ring_bytes / slots holds fewer than 256 rows. */
+B2_API int b2_debug_stream_plan(int64_t n, int32_t d, int32_t dtype, int64_t ring_bytes, int64_t* chunk_rows, int64_t* n_chunks,
+                                int32_t* slots);
+/* CUDA-event times (ms) of the last search of a host-resident index: out4[0] the host-to-device copies (copy stream),
+ * [1] the span of the streamed filter on the search stream (first chunk wait to last fold), [2] the filter launches, [3]
+ * finalize. [1] - [2] is the part of the pipeline not spent in the filter: copies the filter did not hide, plus the folds. */
+B2_API int b2_debug_stream_times(const b2_index* idx, float* out4);
 /* The filter's error model for one operand combination (no device work): |filter score - exact inner product| <=
  * rel_eps * |q| * |x| + abs_eps * (|q| + |x|) for a store of `store_dtype` filtered as `filt_dtype` (B2_F32 = tf32 wgmma,
  * B2_BF16 / B2_F16 = 2-byte wgmma) with queries of `q_dtype`, dimension d. abs_eps is non-zero only where an operand is
@@ -227,7 +254,8 @@ B2_API int b2_debug_filter_eps(int32_t store_dtype, int32_t filt_dtype, int32_t 
 /* ---- instrumentation ---------------------------------------------------------------------------------- */
 /* counters since the last b2_stats_reset(): [0] kernels launched by this library, [1] queries answered,
  * [2] queries that took the exact dense fallback, [3] wgmma filter launches, [4] rows rescored exactly,
- * [5] queries of fp32 indexes that the bf16 first-level filter could not certify and the tf32 level answered.
+ * [5] queries of fp32 indexes that the bf16 first-level filter could not certify and the tf32 level answered,
+ * [6] bytes copied host-to-device by searches of host-resident indexes, [7] corpus chunks those searches filtered.
  * Returns how many counters were written (<= cap). */
 B2_API int b2_stats(int64_t* out, int32_t cap);
 B2_API void b2_stats_reset(void);

@@ -23,7 +23,8 @@ SYMBOLS = [
     "b2_index_ntotal", "b2_index_dim", "b2_index_dtype", "b2_index_metric", "b2_index_device", "b2_index_data_dev",
     "b2_index_search", "b2_index_search_dev", "b2_merge_topk_dev", "b2_index_search_packed_dev", "b2_merge_topk_packed_dev", "b2_index_search_stage1_dev", "b2_index_search_stage2_packed_dev", "b2_index_gather", "b2_threshold_pairs",
     "b2_connected_components", "b2_kmeans", "b2_kmeans_assign", "b2_kmeans_accumulate", "b2_kmeans_assign_dev", "b2_kmeans_accumulate_dev", "b2_stats", "b2_stats_reset", "b2_last_filter_ms", "b2_host_f32_to_bf16", "b2_host_bf16_to_f32", "b2_debug_filter_plan",
-    "b2_debug_filter_lists", "b2_debug_filter_eps",
+    "b2_debug_filter_lists", "b2_debug_filter_eps", "b2_index_create_host", "b2_index_resident", "b2_debug_stream_plan",
+    "b2_debug_stream_times",
 ]
 
 
@@ -54,6 +55,14 @@ def lib() -> ctypes.CDLL:
     L.b2_max_k.restype = c.c_int
     L.b2_index_create.restype = c.c_int
     L.b2_index_create.argtypes = [vp, i64, i32, i32, i32, i32, i32, c.POINTER(vp)]
+    L.b2_index_create_host.restype = c.c_int
+    L.b2_index_create_host.argtypes = [vp, i64, i32, i32, i32, i32, i64, c.POINTER(vp)]
+    L.b2_index_resident.restype = i32
+    L.b2_index_resident.argtypes = [vp]
+    L.b2_debug_stream_plan.restype = c.c_int
+    L.b2_debug_stream_plan.argtypes = [i64, i32, i32, i64, c.POINTER(i64), c.POINTER(i64), c.POINTER(i32)]
+    L.b2_debug_stream_times.restype = c.c_int
+    L.b2_debug_stream_times.argtypes = [vp, c.POINTER(f32)]
     L.b2_index_free.restype = None
     L.b2_index_free.argtypes = [vp]
     for name, rt in [("b2_index_ntotal", i64), ("b2_index_dim", i32), ("b2_index_dtype", i32),
@@ -144,7 +153,15 @@ def stats() -> dict:
     buf = (ctypes.c_int64 * 8)()
     lib().b2_stats(buf, 8)
     return {"launches": buf[0], "queries": buf[1], "fallback_queries": buf[2], "filter_launches": buf[3],
-            "rescored_rows": buf[4], "second_level_queries": buf[5]}
+            "rescored_rows": buf[4], "second_level_queries": buf[5], "streamed_bytes": buf[6], "streamed_chunks": buf[7]}
+
+
+def stream_plan(n: int, d: int, dtype: int, ring_bytes: int = 0) -> dict:
+    """Chunking of a host-resident index (host logic only, no device needed): chunk_rows, n_chunks, slots. Chunk c owns the
+    rows [c * chunk_rows, min(n, (c + 1) * chunk_rows)) and streams chunk_rows rows from min(c * chunk_rows, n - chunk_rows)."""
+    rows, nc, slots = ctypes.c_int64(), ctypes.c_int64(), ctypes.c_int32()
+    check(lib().b2_debug_stream_plan(n, d, dtype, ring_bytes, ctypes.byref(rows), ctypes.byref(nc), ctypes.byref(slots)))
+    return {"chunk_rows": rows.value, "n_chunks": nc.value, "slots": slots.value}
 
 
 def stats_reset() -> None:
@@ -216,9 +233,15 @@ class Index:
     """Owning wrapper of a b2_index handle."""
 
     def __init__(self, x, dtype: int, metric: int = METRIC_IP, device: int = 0, on_device_ptr: Optional[int] = None,
-                 n: Optional[int] = None, d: Optional[int] = None):
+                 n: Optional[int] = None, d: Optional[int] = None, residency: str = "device", ring_bytes: int = 0):
+        """residency="host": the rows stay in pinned host memory and searches stream them through a device ring of ring_bytes
+        (0 = the library default); x must then be a host array."""
         L = lib()
         self._h = ctypes.c_void_p()
+        if residency not in ("device", "host"):
+            raise ValueError("residency must be 'device' or 'host'")
+        if residency == "host" and on_device_ptr is not None:
+            raise ValueError("a host-resident index is built from a host array")
         if on_device_ptr is not None:
             assert n is not None and d is not None
             check(L.b2_index_create(ctypes.c_void_p(on_device_ptr), n, d, dtype, metric, device, 1, ctypes.byref(self._h)))
@@ -232,7 +255,10 @@ class Index:
             if x.ndim != 2:
                 raise ValueError("matrix must be 2-D")
             n, d = x.shape
-            check(L.b2_index_create(_ptr(x) if n else None, n, d, dtype, metric, device, 0, ctypes.byref(self._h)))
+            if residency == "host":
+                check(L.b2_index_create_host(_ptr(x) if n else None, n, d, dtype, metric, device, int(ring_bytes), ctypes.byref(self._h)))
+            else:
+                check(L.b2_index_create(_ptr(x) if n else None, n, d, dtype, metric, device, 0, ctypes.byref(self._h)))
         self.n, self.d, self.dtype, self.metric, self.device = int(n), int(d), dtype, metric, device
 
     def close(self) -> None:
@@ -249,6 +275,17 @@ class Index:
     @property
     def handle(self):
         return self._h
+
+    @property
+    def resident(self) -> str:
+        """Where the rows live: "device" or "host"."""
+        return "host" if lib().b2_index_resident(self._h) == 1 else "device"
+
+    def stream_times(self) -> dict:
+        """CUDA-event times (ms) of the last search of a host-resident index (b2_debug_stream_times)."""
+        t = (ctypes.c_float * 4)()
+        check(lib().b2_debug_stream_times(self._h, t))
+        return {"copy_ms": t[0], "span_ms": t[1], "filter_ms": t[2], "finalize_ms": t[3]}
 
     @property
     def data_ptr(self) -> int:

@@ -31,6 +31,12 @@ using namespace b2;
 
 namespace b2 {
 
+// fp32 stores of at least 4096 rows keep a bf16 copy for the first level of a two-level search (B2_F32_BF16_FIRST=0: no copy)
+static bool f32_bf16_first() {
+    static const bool on = [] { const char* e = getenv("B2_F32_BF16_FIRST"); return e ? atoi(e) != 0 : true; }();
+    return on;
+}
+
 // Build the searchable view of a row-major matrix that already sits in device memory.
 int build_view(const void* store, int64_t n, int d, int dtype, DevBuf& filt_pad, DevBuf& norm2, DevBuf& scalar,
                       MatView& v, cudaStream_t st, DevBuf* filt16) {
@@ -53,8 +59,7 @@ int build_view(const void* store, int64_t n, int d, int dtype, DevBuf& filt_pad,
     v.filt16_pitch = 0;
     v.filt_f16 = nullptr;
     v.filt_f16_pitch = 0;
-    static const bool bf16_first = [] { const char* e = getenv("B2_F32_BF16_FIRST"); return e ? atoi(e) != 0 : true; }();
-    if (filt16 && dtype == B2_F32 && bf16_first && n >= 4096) {
+    if (filt16 && dtype == B2_F32 && f32_bf16_first() && n >= 4096) {
         v.filt16_pitch = round_up(d, 8);
         B2_TRY(filt16->ensure((size_t)n * v.filt16_pitch * 2));
         B2_TRY(launch_convert_pad(store, dtype, n, d, filt16->p, B2_BF16, v.filt16_pitch, st));
@@ -372,14 +377,15 @@ static int adapt_queries(b2_index* idx, const void*& q, int32_t& q_dtype, int64_
         q = idx->q_wide.p;
         q_dtype = wide;
     }
-    if (q_dtype != B2_I8) B2_TRY(ensure_f16_copy(idx->view, idx->filt_f16, st));
+    // (a host-resident index converts each streamed chunk instead)
+    if (q_dtype != B2_I8 && !idx->host) B2_TRY(ensure_f16_copy(idx->view, idx->filt_f16, st));
     return B2_OK;
 }
 
 // searchable view for an ids subset (faiss_vs.py:57-64: temporary index over vecs[ids])
 static int build_subset(b2_index* idx, const int64_t* ids_dev, int64_t m, int q_dtype, MatView& sub, cudaStream_t st) {
     B2_TRY(idx->sub_store.ensure((size_t)std::max<int64_t>(m, 1) * idx->d * esize(idx->dtype)));
-    B2_TRY(gather_rows_checked(idx->store.p, idx->dtype, idx->d, ids_dev, m, idx->n, idx->sub_store.p, idx->scalar, st));
+    B2_TRY(gather_rows_checked(idx->view.store, idx->dtype, idx->d, ids_dev, m, idx->n, idx->sub_store.p, idx->scalar, st));
     B2_TRY(build_view(idx->sub_store.p, m, idx->d, idx->dtype, idx->sub_filt, idx->sub_norm2, idx->scalar, sub, st, &idx->sub_filt16));
     return q_dtype != B2_I8 ? ensure_f16_copy(sub, idx->sub_filt_f16, st) : B2_OK;
 }
@@ -404,6 +410,344 @@ static void for_each_chunk(int64_t count, const Body& body) {
     for (auto& t : pool) t.join();
 }
 
+// ---- host-resident indexes ------------------------------------------------------------------------------------------------
+// The rows stay in pinned, mapped host memory. A search streams them in chunks through a ring of device slots on a copy stream
+// owned by the handle, filters every chunk with the unchanged filter kernel, folds the chunk's lists into running per-query
+// lists (fold_lists_kernel) and certifies once at the end; finalize and the dense path read the rows through the mapped
+// pointer. Norms stay on the device.
+
+constexpr size_t kDefaultRingBytes = 1ull << 30;
+
+// device bytes one streamed row takes in the ring: the filter-ready row (TMA pitch), plus its fp16 form for an int8 store
+static size_t ring_row_bytes(int d, int dtype) {
+    size_t b = (size_t)round_up(d, tma_align_elems(dtype)) * esize(dtype);
+    if (dtype == B2_I8) b += (size_t)round_up(d, tma_align_elems(B2_F16)) * 2;
+    return b;
+}
+
+// Chunks of a corpus of n rows for a ring of ring_bytes (0 = the default) of HostStore::SLOTS slots: chunk c owns the rows
+// [c * rows, min(n, (c + 1) * rows)) and streams the `rows` rows from min(c * rows, n - rows) on, so every chunk has the same
+// shape (and the same filter plan); the last one re-streams the tail of its predecessor and the fold skips those rows.
+static int stream_plan(int64_t n, int d, int dtype, size_t ring_bytes, int64_t* chunk_rows, int* n_chunks) {
+    const size_t rb = ring_bytes ? ring_bytes : kDefaultRingBytes;
+    const size_t row = ring_row_bytes(d, dtype);
+    const int64_t cap = (int64_t)(rb / ((size_t)HostStore::SLOTS * row)) / 256 * 256;
+    if (cap < 256) {
+        set_error("ring_bytes=%zu holds fewer than 256 rows per slot (%d slots, %zu bytes per row)", rb, HostStore::SLOTS, row);
+        return B2_EINVAL;
+    }
+    if (n <= cap) {
+        *chunk_rows = n;
+        *n_chunks = n > 0 ? 1 : 0;
+        return B2_OK;
+    }
+    const int64_t nc = ceil_div(n, cap);
+    const int64_t rows = std::min<int64_t>(cap, round_up(ceil_div(n, nc), 256));  // balanced: the overlap stays below 256 nc
+    *chunk_rows = rows;
+    *n_chunks = (int)ceil_div(n, rows);
+    return B2_OK;
+}
+
+// norms (canonical, per row: bit for bit those of a device build), max norm, bf16 copy and plan of rows already in H.rows
+static int host_rows_init(HostRows& H, int64_t n, int d, int dtype, size_t ring_bytes, cudaStream_t st) {
+    H.n = n;
+    H.d = d;
+    H.dtype = dtype;
+    B2_TRY(stream_plan(n, d, dtype, ring_bytes, &H.chunk_rows, &H.n_chunks));
+    if (dtype == B2_F32 && f32_bf16_first() && n >= 4096) {
+        B2_TRY(H.rows16.ensure((size_t)n * d * 2));
+        B2_TRY(b2_host_f32_to_bf16(reinterpret_cast<const float*>(H.rows.p), n * d, reinterpret_cast<uint16_t*>(H.rows16.p), nullptr));
+    }
+    B2_TRY(H.norm2.ensure((size_t)std::max<int64_t>(n, 1) * (dtype == B2_I8 ? 2 : 1) * sizeof(float)));
+    B2_TRY(H.scalar.ensure(64));
+    B2_TRY(launch_row_norms(H.rows.dev, dtype, n, d, H.norm2.as<float>(), H.scalar.as<float>(), st));
+    if (dtype == B2_I8)
+        B2_TRY(launch_row_norms_i8(H.rows.dev, n, d, reinterpret_cast<int32_t*>(H.norm2.as<float>() + std::max<int64_t>(n, 1)), st));
+    B2_CUDA(cudaMemcpyAsync(&H.max_norm, H.scalar.p, sizeof(float), cudaMemcpyDeviceToHost, st));
+    B2_CUDA(cudaStreamSynchronize(st));
+    return B2_OK;
+}
+
+// the view finalize, the dense path and gathers read: the rows through the mapped pointer, the device norms
+static MatView host_view(HostRows& H) {
+    MatView v;
+    v.store = H.rows.dev;
+    v.n = H.n;
+    v.d = H.d;
+    v.dtype = v.filt_dtype = H.dtype;
+    v.filt_pitch = round_up(H.d, tma_align_elems(H.dtype));
+    v.norm2 = H.norm2.as<float>();
+    v.norm2_i8 = H.dtype == B2_I8 ? reinterpret_cast<const int32_t*>(H.norm2.as<float>() + std::max<int64_t>(H.n, 1)) : nullptr;
+    v.max_norm = H.max_norm;
+    return v;
+}
+
+// The filter plan of one chunk (every chunk streams chunk_rows rows, so one plan serves them all). Level 1 (the second level of
+// an fp32 store) streams the fp32 rows; level 0 of an fp32 store streams the bf16 copy when the plan takes two levels.
+static int host_plan(b2_index* idx, HostRows& H, const void* q_dev, int q_dtype, int64_t nq, int k, int level, FilterPlan& p) {
+    MatView Xc = host_view(H);
+    Xc.n = H.chunk_rows;
+    if (level == 0 && H.rows16.p) {
+        Xc.filt16 = H.rows16.dev;  // (the plan only tests it; each chunk's slot replaces it)
+        Xc.filt16_pitch = round_up(H.d, tma_align_elems(B2_BF16));
+    }
+    if (H.dtype == B2_I8 && q_dtype != B2_I8) {
+        Xc.filt_f16 = H.rows.dev;  // (likewise: each chunk's fp16 form replaces it)
+        Xc.filt_f16_pitch = round_up(H.d, tma_align_elems(B2_F16));
+    }
+    return plan_filter(Xc, q_dev, q_dtype, nq, k, false, idx->device, p);
+}
+
+static int ensure_events(std::vector<cudaEvent_t>& ev, size_t count) {
+    while (ev.size() < count) {
+        cudaEvent_t e = nullptr;
+        B2_CUDA(cudaEventCreate(&e));
+        ev.push_back(e);
+    }
+    return B2_OK;
+}
+
+// Filter the query chunk qc of plan p over every corpus chunk of H (copy of chunk c + 1 on the copy stream while chunk c is
+// filtered) and fold the lists into hs.run_* ([qc.nq, cap] and [qc.nq]).
+static int stream_filter_fold(b2_index* idx, HostRows& H, const FilterPlan& p, const FilterChunk& qc, int metric, int cap,
+                              cudaStream_t st) {
+    HostStore& hs = *idx->host;
+    const int d = H.d;
+    const bool via_f16 = p.X.filt_dtype == B2_F16 && H.dtype == B2_I8;  // float queries on an int8 store
+    const int src_dtype = p.two_level ? B2_BF16 : H.dtype;
+    const char* src = reinterpret_cast<const char*>(p.two_level ? H.rows16.p : H.rows.p);
+    const size_t src_row = (size_t)d * esize(src_dtype);
+    const size_t slot_pitch = via_f16 ? src_row : (size_t)p.X.filt_pitch * esize(src_dtype);
+    const int64_t R = H.chunk_rows;
+    for (int s = 0; s < HostStore::SLOTS; ++s) {
+        B2_TRY(hs.slot[s].ensure((size_t)R * slot_pitch));
+        if (via_f16) B2_TRY(hs.slot16[s].ensure((size_t)R * p.X.filt_pitch * 2));
+    }
+    // the queries in the filter's form, once for every corpus chunk
+    FilterPlan pc = p;
+    FilterChunk c = qc;
+    c.q0 = 0;
+    const void* qsrc = reinterpret_cast<const char*>(p.q) + (size_t)qc.q0 * d * esize(p.q_dtype);
+    pc.q = qsrc;
+    if (!p.q_in_place) {
+        B2_TRY(idx->q_filt.ensure((size_t)qc.nq * p.q_pitch * esize(p.X.filt_dtype)));
+        B2_TRY(launch_prep_queries(qsrc, p.q_dtype, qc.nq, d, idx->q_filt.p, p.X.filt_dtype, p.q_pitch, st));
+        pc.q = idx->q_filt.p;
+        pc.q_in_place = true;
+    }
+    B2_TRY(hs.run_score.ensure((size_t)qc.nq * cap * sizeof(float)));
+    B2_TRY(hs.run_id.ensure((size_t)qc.nq * cap * sizeof(int32_t)));
+    B2_TRY(hs.run_thr.ensure((size_t)qc.nq * sizeof(float)));
+    B2_CUDA(cudaMemsetAsync(hs.run_id.p, 0xFF, (size_t)qc.nq * cap * sizeof(int32_t), st));
+    B2_TRY(launch_fill_f32(hs.run_thr.as<float>(), qc.nq, -INFINITY, st));
+    const int nc = H.n_chunks;
+    B2_TRY(ensure_events(hs.ev, (size_t)4 * nc));
+    auto issue_copy = [&](int ch) -> int {
+        const int s = ch % HostStore::SLOTS;
+        const int64_t base = std::min<int64_t>((int64_t)ch * R, H.n - R);
+        B2_CUDA(cudaStreamWaitEvent(hs.copy, hs.freed[s], 0));  // the slot's previous chunk has been filtered
+        B2_CUDA(cudaEventRecord(hs.ev[4 * ch], hs.copy));
+        B2_CUDA(cudaMemcpy2DAsync(hs.slot[s].p, slot_pitch, src + (size_t)base * src_row, src_row, src_row, (size_t)R,
+                                  cudaMemcpyHostToDevice, hs.copy));
+        B2_CUDA(cudaEventRecord(hs.ev[4 * ch + 1], hs.copy));
+        B2_CUDA(cudaEventRecord(hs.copied[s], hs.copy));
+        g_stats[ST_STREAM_BYTES] += R * (int64_t)src_row;
+        return B2_OK;
+    };
+    B2_CUDA(cudaEventRecord(hs.span0, st));
+    B2_TRY(issue_copy(0));
+    for (int ch = 0; ch < nc; ++ch) {
+        if (ch + 1 < nc) B2_TRY(issue_copy(ch + 1));
+        const int s = ch % HostStore::SLOTS;
+        const int64_t base = std::min<int64_t>((int64_t)ch * R, H.n - R);
+        B2_CUDA(cudaStreamWaitEvent(st, hs.copied[s], 0));
+        pc.X = p.X;
+        if (via_f16) {
+            B2_TRY(launch_convert_pad(hs.slot[s].p, B2_I8, R, d, hs.slot16[s].p, B2_F16, p.X.filt_pitch, st));
+            pc.X.filt = hs.slot16[s].p;
+        } else {
+            pc.X.filt = hs.slot[s].p;
+        }
+        pc.X.store = pc.X.filt;
+        pc.X.norm2 = p.X.norm2 + base;
+        pc.X.norm2_i8 = p.X.norm2_i8 ? p.X.norm2_i8 + base : nullptr;
+        B2_CUDA(cudaEventRecord(hs.ev[4 * ch + 2], st));
+        B2_TRY(run_filter(idx, pc, c, metric, st));
+        B2_CUDA(cudaEventRecord(hs.ev[4 * ch + 3], st));
+        B2_CUDA(cudaEventRecord(hs.freed[s], st));  // the slot may take its next chunk
+        B2_TRY(launch_fold_lists(idx->cand_score.as<float>(), idx->cand_id.as<int32_t>(), idx->cand_thr.as<float>(), c.nq,
+                                 2 * c.n_splits, p.kp / 2, base, (int64_t)ch * R - base, cap, hs.run_score.as<float>(),
+                                 hs.run_id.as<int32_t>(), hs.run_thr.as<float>(), st));
+        g_stats[ST_STREAM_CHUNKS]++;
+    }
+    B2_CUDA(cudaEventRecord(hs.span1, st));
+    return B2_OK;
+}
+
+// event times of the last stream_filter_fold (after the search stream was synchronised)
+static void stream_times_add(b2_index* idx, int nc) {
+    HostStore& hs = *idx->host;
+    float ms = 0.f, filt = 0.f;
+    for (int ch = 0; ch < nc; ++ch) {
+        if (cudaEventElapsedTime(&ms, hs.ev[4 * ch], hs.ev[4 * ch + 1]) == cudaSuccess) hs.copy_ms += ms;
+        if (cudaEventElapsedTime(&ms, hs.ev[4 * ch + 2], hs.ev[4 * ch + 3]) == cudaSuccess) filt += ms;
+    }
+    if (cudaEventElapsedTime(&ms, hs.span0, hs.span1) == cudaSuccess) hs.span_ms += ms;
+    hs.filter_ms += filt;
+    idx->last_filter_ms = (idx->last_filter_ms < 0 ? 0.f : idx->last_filter_ms) + filt;
+}
+
+// The streamed search of the rows H (level as in search_core: level 1 is the tf32 second level of an fp32 store, which streams
+// the fp32 rows). Results are those of search_core over the same rows in device memory, bit for bit.
+static int stream_search(b2_index* idx, HostRows& H, int metric, const void* q_dev, int q_dtype, int64_t nq, int k,
+                         const int64_t* id_map, int64_t id_offset, float* out_sc, int64_t* out_id, cudaStream_t st, int level) {
+    HostStore& hs = *idx->host;
+    if (level == 0) {
+        idx->last_filter_ms = -1.f;
+        hs.copy_ms = hs.span_ms = hs.filter_ms = hs.finalize_ms = 0.f;
+    }
+    if (nq <= 0) return B2_OK;
+    if (level == 0) g_stats[ST_QUERIES] += nq;
+    if (H.n <= 0) {
+        fill_pad_kernel<<<132, 256, 0, st>>>(out_sc, out_id, nq * k, metric == B2_METRIC_L2 ? FLT_MAX : -FLT_MAX);
+        B2_LAUNCH_CHECK();
+        return B2_OK;
+    }
+    const MatView Xw = host_view(H);
+    FilterPlan p;
+    B2_TRY(host_plan(idx, H, q_dev, q_dtype, nq, k, level, p));
+    const int cap = p.use_filter ? finalize_capacity(p.kp, k) : 0;
+    if (!p.use_filter || cap == 0) {
+        // the dense path over every row, read through the mapped pointer
+        if (k > dense_max_k()) {
+            set_error("k=%d is not supported (max %d)", k, dense_max_k());
+            return B2_ERANGE;
+        }
+        const bool full_sort = k > dense_select_max_k();
+        const int64_t rows = std::min<int64_t>(dense_rows_cap(Xw.n, full_sort), nq);
+        B2_TRY(idx->dense.ensure((size_t)rows * Xw.n * sizeof(float)));
+        if (full_sort) B2_TRY(idx->sort_keys.ensure(dense_sort_ws_bytes(rows, Xw.n)));
+        B2_TRY(launch_dense_topk(Xw, q_dev, q_dtype, nq, nullptr, nq, metric, k, id_map, id_offset, idx->dense.as<float>(), rows,
+                                 full_sort ? idx->sort_keys.as<uint64_t>() : nullptr, out_sc, out_id, st));
+        g_stats[ST_FALLBACK] += nq;
+        return B2_OK;
+    }
+    int64_t n_deferred = 0;
+    for (const FilterChunk& qc : p.chunks) {
+        B2_TRY(stream_filter_fold(idx, H, p, qc, metric, cap, st));
+        const void* qc_ptr = reinterpret_cast<const char*>(q_dev) + (size_t)qc.q0 * H.d * esize(q_dtype);
+        float* osc = out_sc + (size_t)qc.q0 * k;
+        int64_t* oid = out_id + (size_t)qc.q0 * k;
+        B2_TRY(idx->flags.ensure((size_t)qc.nq * sizeof(int32_t)));
+        B2_TRY(idx->sel.ensure((size_t)(qc.nq + 1) * sizeof(int32_t)));
+        B2_TRY(idx->h_flags.ensure(64));
+        int32_t* sel_count = idx->sel.as<int32_t>();
+        int32_t* sel_list = sel_count + 1;
+        B2_CUDA(cudaMemsetAsync(sel_count, 0, sizeof(int32_t), st));
+        B2_CUDA(cudaEventRecord(hs.fin0, st));
+        B2_TRY(launch_finalize(Xw, qc_ptr, q_dtype, qc.nq, metric, k, p.kp, cap, 1, hs.run_score.as<float>(), hs.run_id.as<int32_t>(),
+                               hs.run_thr.as<float>(), p.rel_eps, p.abs_eps, p.q_norm_limit, id_map, id_offset, osc, oid,
+                               idx->flags.as<int32_t>(), sel_list, sel_count, st, nullptr));
+        B2_CUDA(cudaEventRecord(hs.fin1, st));
+        int32_t* h_count = reinterpret_cast<int32_t*>(idx->h_flags.p);
+        B2_CUDA(cudaMemcpyAsync(h_count, sel_count, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+        cudaError_t se = cudaStreamSynchronize(st);
+        if (se != cudaSuccess) {
+            set_error("streamed search failed on the device: %s", cudaGetErrorString(se));
+            return B2_ECUDA;
+        }
+        stream_times_add(idx, H.n_chunks);
+        float ms = 0.f;
+        if (cudaEventElapsedTime(&ms, hs.fin0, hs.fin1) == cudaSuccess) hs.finalize_ms += ms;
+        const int64_t n_sel = *h_count;
+        if (n_sel == 0) continue;
+        if (p.two_level) {
+            B2_TRY(idx->defer.ensure((size_t)nq * sizeof(int64_t)));
+            defer_append_kernel<<<(unsigned)ceil_div(n_sel, 256), 256, 0, st>>>(sel_list, n_sel, qc.q0, idx->defer.as<int64_t>() + n_deferred);
+            B2_LAUNCH_CHECK();
+            n_deferred += n_sel;
+            continue;
+        }
+        // exact dense path for the queries the certificate could not cover
+        g_stats[ST_FALLBACK] += n_sel;
+        const int64_t rows = std::min<int64_t>(dense_rows_cap(Xw.n, false), n_sel);
+        B2_TRY(idx->dense.ensure((size_t)rows * Xw.n * sizeof(float)));
+        B2_TRY(launch_dense_topk(Xw, qc_ptr, q_dtype, qc.nq, sel_list, n_sel, metric, k, id_map, id_offset, idx->dense.as<float>(), rows,
+                                 nullptr, osc, oid, st));
+    }
+    if (n_deferred > 0) {
+        // second level: the deferred queries against the tf32 filter over the streamed fp32 rows
+        const size_t qrow = (size_t)H.d * esize(q_dtype);
+        B2_TRY(idx->q_sub.ensure((size_t)n_deferred * qrow));
+        B2_TRY(idx->sub_sc.ensure((size_t)n_deferred * k * sizeof(float)));
+        B2_TRY(idx->sub_id.ensure((size_t)n_deferred * k * sizeof(int64_t)));
+        B2_TRY(idx->scalar.ensure(64));
+        int* err = reinterpret_cast<int*>(idx->scalar.as<char>() + 16);
+        B2_TRY(launch_gather_rows(q_dev, q_dtype, H.d, idx->defer.as<int64_t>(), n_deferred, nq, idx->q_sub.p, err, st));
+        B2_TRY(stream_search(idx, H, metric, idx->q_sub.p, q_dtype, n_deferred, k, id_map, id_offset, idx->sub_sc.as<float>(),
+                             idx->sub_id.as<int64_t>(), st, /*level=*/1));
+        scatter_rows_kernel<<<(unsigned)ceil_div(n_deferred * k, 256), 256, 0, st>>>(idx->defer.as<int64_t>(), n_deferred, k,
+                                                                                    idx->sub_sc.as<float>(), idx->sub_id.as<int64_t>(),
+                                                                                    out_sc, out_id);
+        B2_LAUNCH_CHECK();
+        g_stats[ST_SECOND_LEVEL] += n_deferred;
+    }
+    return B2_OK;
+}
+
+// A search of a host-resident index: the whole index, or an ids subset (ids_host and / or ids_dev; ids_dev is what the results
+// map through). A subset whose rows fit in the ring is gathered from host memory into a device view and searched as on a
+// device-resident index; a larger one is gathered on the host, by threads, into pinned staging and streamed.
+static int host_search(b2_index* idx, const void* q_dev, int q_dtype, int64_t nq, int k, const int64_t* ids_host, const int64_t* ids_dev,
+                       int64_t n_ids, int64_t id_offset, float* out_sc, int64_t* out_id, cudaStream_t st) {
+    HostStore& hs = *idx->host;
+    if (!ids_dev) return stream_search(idx, hs.main, idx->metric, q_dev, q_dtype, nq, k, nullptr, id_offset, out_sc, out_id, st, 0);
+    if ((size_t)n_ids * ring_row_bytes(idx->d, idx->dtype) <= hs.ring_bytes) {
+        MatView sub;
+        B2_TRY(build_subset(idx, ids_dev, n_ids, q_dtype, sub, st));
+        return search_core(idx, sub, idx->metric, q_dev, q_dtype, nq, k, ids_dev, 0, out_sc, out_id, st);
+    }
+    if (!ids_host) {
+        B2_TRY(hs.staging_ids.ensure((size_t)n_ids * sizeof(int64_t)));
+        B2_CUDA(cudaMemcpyAsync(hs.staging_ids.p, ids_dev, (size_t)n_ids * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+        B2_CUDA(cudaStreamSynchronize(st));
+        ids_host = reinterpret_cast<const int64_t*>(hs.staging_ids.p);
+    }
+    for (int64_t i = 0; i < n_ids; ++i) {
+        if (ids_host[i] < 0 || ids_host[i] >= idx->n) {
+            set_error("ids contains a position outside [0, %lld)", (long long)idx->n);
+            return B2_ERANGE;
+        }
+    }
+    if (!hs.sub) hs.sub.reset(new HostRows());
+    HostRows& S = *hs.sub;
+    const size_t row = (size_t)idx->d * esize(idx->dtype);
+    B2_TRY(S.rows.ensure((size_t)n_ids * row));
+    const char* src = reinterpret_cast<const char*>(hs.main.rows.p);
+    char* dst = reinterpret_cast<char*>(S.rows.p);
+    for_each_chunk(n_ids, [&](int64_t lo, int64_t hi) {
+        for (int64_t i = lo; i < hi; ++i) memcpy(dst + (size_t)i * row, src + (size_t)ids_host[i] * row, row);
+    });
+    B2_TRY(host_rows_init(S, n_ids, idx->d, idx->dtype, hs.ring_bytes, st));
+    return stream_search(idx, S, idx->metric, q_dev, q_dtype, nq, k, ids_dev, 0, out_sc, out_id, st, 0);
+}
+
+}  // namespace b2
+
+namespace b2 {
+HostStore::~HostStore() {
+    if (copy) {
+        cudaStreamSynchronize(copy);
+        cudaStreamDestroy(copy);
+    }
+    for (int s = 0; s < SLOTS; ++s) {
+        if (copied[s]) cudaEventDestroy(copied[s]);
+        if (freed[s]) cudaEventDestroy(freed[s]);
+    }
+    for (cudaEvent_t e : ev) cudaEventDestroy(e);
+    for (cudaEvent_t e : {span0, span1, fin0, fin1})
+        if (e) cudaEventDestroy(e);
+}
 }  // namespace b2
 
 namespace b2 {
@@ -458,8 +802,8 @@ int b2_device_count(void) {
 
 int b2_max_k(void) { return dense_max_k(); }
 
-int b2_index_create(const void* x, int64_t n, int32_t d, int32_t dtype, int32_t metric, int32_t device, int32_t x_on_device,
-                    b2_index** out) {
+// the checks both create entry points make before any device work
+static int check_create_args(const void* x, int64_t n, int32_t d, int32_t dtype, int32_t metric, b2_index** out) {
     if (!out) { set_error("out is NULL"); return B2_EINVAL; }
     *out = nullptr;
     if (n < 0 || d <= 0 || (n > 0 && !x)) { set_error("bad matrix shape n=%lld d=%d", (long long)n, d); return B2_EINVAL; }
@@ -470,6 +814,10 @@ int b2_index_create(const void* x, int64_t n, int32_t d, int32_t dtype, int32_t 
         return B2_EINVAL;
     }
     if (metric != B2_METRIC_IP && metric != B2_METRIC_L2) { set_error("metric must be B2_METRIC_IP or B2_METRIC_L2"); return B2_EINVAL; }
+    return B2_OK;
+}
+
+static int check_create_device(int32_t device) {
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
         cudaGetLastError();
@@ -481,6 +829,13 @@ int b2_index_create(const void* x, int64_t n, int32_t d, int32_t dtype, int32_t 
     cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device);
     cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, device);
     if (major != 9 || minor != 0) { set_error("device %d is sm_%d%d; this library is built for sm_90a (H100) only", device, major, minor); return B2_ENODEV; }
+    return B2_OK;
+}
+
+int b2_index_create(const void* x, int64_t n, int32_t d, int32_t dtype, int32_t metric, int32_t device, int32_t x_on_device,
+                    b2_index** out) {
+    B2_TRY(check_create_args(x, n, d, dtype, metric, out));
+    B2_TRY(check_create_device(device));
     DeviceGuard guard(device);
     b2_index* idx = new b2_index();
     idx->device = device;
@@ -514,6 +869,57 @@ int b2_index_create(const void* x, int64_t n, int32_t d, int32_t dtype, int32_t 
     return B2_OK;
 }
 
+int b2_index_create_host(const void* x, int64_t n, int32_t d, int32_t dtype, int32_t metric, int32_t device, int64_t ring_bytes,
+                         b2_index** out) {
+    B2_TRY(check_create_args(x, n, d, dtype, metric, out));
+    if (n >= (1LL << 31)) { set_error("a host-resident index holds fewer than 2^31 rows (got %lld): its row ids are int32", (long long)n); return B2_EINVAL; }
+    if (ring_bytes < 0) { set_error("ring_bytes < 0"); return B2_EINVAL; }
+    {
+        int64_t rows = 0;
+        int nc = 0;
+        B2_TRY(stream_plan(n, d, dtype, (size_t)ring_bytes, &rows, &nc));
+    }
+    B2_TRY(check_create_device(device));
+    DeviceGuard guard(device);
+    b2_index* idx = new b2_index();
+    idx->device = device;
+    idx->n = n;
+    idx->d = d;
+    idx->dtype = dtype;
+    idx->metric = metric;
+    idx->host.reset(new HostStore());
+    HostStore& hs = *idx->host;
+    hs.ring_bytes = ring_bytes ? (size_t)ring_bytes : kDefaultRingBytes;
+    auto fail = [&](int rc) { b2_index_free(idx); return rc; };
+    bool ok = cudaStreamCreateWithFlags(&idx->stream, cudaStreamNonBlocking) == cudaSuccess &&
+              cudaStreamCreateWithFlags(&hs.copy, cudaStreamNonBlocking) == cudaSuccess && cudaEventCreate(&idx->ev0) == cudaSuccess &&
+              cudaEventCreate(&idx->ev1) == cudaSuccess;
+    for (int s = 0; ok && s < HostStore::SLOTS; ++s)
+        ok = cudaEventCreateWithFlags(&hs.copied[s], cudaEventDisableTiming) == cudaSuccess &&
+             cudaEventCreateWithFlags(&hs.freed[s], cudaEventDisableTiming) == cudaSuccess;
+    for (cudaEvent_t* e : {&hs.span0, &hs.span1, &hs.fin0, &hs.fin1}) ok = ok && cudaEventCreate(e) == cudaSuccess;
+    if (!ok) {
+        set_error("stream/event creation failed: %s", cudaGetErrorString(cudaGetLastError()));
+        return fail(B2_ECUDA);
+    }
+    const size_t bytes = (size_t)n * d * esize(dtype);
+    int rc = hs.main.rows.ensure(std::max<size_t>(bytes, 1));
+    if (rc != B2_OK) return fail(rc);
+    const char* src = reinterpret_cast<const char*>(x);
+    char* dst = reinterpret_cast<char*>(hs.main.rows.p);
+    for_each_chunk((int64_t)ceil_div((int64_t)bytes, 1 << 12), [&](int64_t lo, int64_t hi) {  // threaded copy, 4 KB pages
+        const size_t b0 = (size_t)lo << 12, b1 = std::min(bytes, (size_t)hi << 12);
+        memcpy(dst + b0, src + b0, b1 - b0);
+    });
+    rc = host_rows_init(hs.main, n, d, dtype, hs.ring_bytes, idx->stream);
+    if (rc != B2_OK) return fail(rc);
+    idx->view = host_view(hs.main);
+    *out = idx;
+    return B2_OK;
+}
+
+int32_t b2_index_resident(const b2_index* idx) { return idx ? (idx->host ? 1 : 0) : -1; }
+
 void b2_index_free(b2_index* idx) {
     if (!idx) return;
     DeviceGuard guard(idx->device);
@@ -525,7 +931,7 @@ int32_t b2_index_dim(const b2_index* idx) { return idx ? idx->d : -1; }
 int32_t b2_index_dtype(const b2_index* idx) { return idx ? idx->dtype : -1; }
 int32_t b2_index_metric(const b2_index* idx) { return idx ? idx->metric : -1; }
 int32_t b2_index_device(const b2_index* idx) { return idx ? idx->device : -1; }
-const void* b2_index_data_dev(const b2_index* idx) { return idx ? idx->store.p : nullptr; }
+const void* b2_index_data_dev(const b2_index* idx) { return idx && !idx->host ? idx->store.p : nullptr; }
 float b2_last_filter_ms(const b2_index* idx) { return idx ? idx->last_filter_ms : -1.f; }
 
 static int check_search_args(b2_index* idx, const void* q, int64_t nq, int32_t q_dtype, int32_t k) {
@@ -545,8 +951,10 @@ int b2_index_search_dev(b2_index* idx, const void* q_dev, int64_t nq, int32_t q_
     DeviceGuard guard(idx->device);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     B2_TRY(adapt_queries(idx, q_dev, q_dtype, nq, st));
-    if (ids_dev) {
-        if (n_ids < 0) { set_error("n_ids < 0"); return B2_EINVAL; }
+    if (ids_dev && n_ids < 0) { set_error("n_ids < 0"); return B2_EINVAL; }
+    if (idx->host) {
+        B2_TRY(host_search(idx, q_dev, q_dtype, nq, k, nullptr, ids_dev, n_ids, id_offset, out_scores_dev, out_idx_dev, st));
+    } else if (ids_dev) {
         MatView sub;
         B2_TRY(build_subset(idx, ids_dev, n_ids, q_dtype, sub, st));
         B2_TRY(search_core(idx, sub, idx->metric, q_dev, q_dtype, nq, k, ids_dev, 0, out_scores_dev, out_idx_dev, st));
@@ -582,7 +990,10 @@ int b2_index_search(b2_index* idx, const void* q, int64_t nq, int32_t q_dtype, i
             ids_dev = idx->ids_dev.as<int64_t>();
         }
     }
-    if (ids_dev) {
+    if (idx->host) {
+        B2_TRY(host_search(idx, q_dev, q_dtype, nq, k, ids_dev ? ids : nullptr, ids_dev, n_ids, 0, idx->out_sc.as<float>(),
+                           idx->out_id.as<int64_t>(), st));
+    } else if (ids_dev) {
         MatView sub;
         B2_TRY(build_subset(idx, ids_dev, n_ids, q_dtype, sub, st));
         B2_TRY(search_core(idx, sub, idx->metric, q_dev, q_dtype, nq, k, ids_dev, 0, idx->out_sc.as<float>(), idx->out_id.as<int64_t>(), st));
@@ -614,6 +1025,7 @@ int b2_index_search_packed_dev(b2_index* idx, const void* q_dev, int64_t nq, int
     B2_TRY(check_search_args(idx, q_dev, nq, q_dtype, k));
     if (nq == 0) return B2_OK;
     if (!out_packed_dev) { set_error("output buffer is NULL"); return B2_EINVAL; }
+    B2_TRY(refuse_host_resident(idx, "b2_index_search_packed_dev"));
     if (idx->n > 0xfffffffeLL) { set_error("packed lists hold 32-bit local ids"); return B2_ERANGE; }
     DeviceGuard guard(idx->device);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
@@ -638,6 +1050,7 @@ int b2_index_search_stage1_dev(b2_index* idx, const void* q_dev, int64_t nq, int
     B2_TRY(check_search_args(idx, q_dev, nq, q_dtype, k));
     if (nq == 0) return B2_OK;
     if (!lower_dev || j <= 0) { set_error("bad stage-1 arguments"); return B2_EINVAL; }
+    B2_TRY(refuse_host_resident(idx, "b2_index_search_stage1_dev"));
     DeviceGuard guard(idx->device);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     B2_TRY(adapt_queries(idx, q_dev, q_dtype, nq, st));
@@ -666,6 +1079,7 @@ int b2_index_search_stage1_dev(b2_index* idx, const void* q_dev, int64_t nq, int
 
 int b2_index_search_stage2_packed_dev(b2_index* idx, const float* hint_dev, uint64_t* out_packed_dev, void* stream) {
     if (!idx) { set_error("Index not loaded"); return B2_EINVAL; }
+    B2_TRY(refuse_host_resident(idx, "b2_index_search_stage2_packed_dev"));
     b2_index::Staged sg = idx->staged;
     idx->staged.active = false;
     if (!sg.active) { set_error("stage 2 without a stage 1"); return B2_EINVAL; }
@@ -705,6 +1119,16 @@ int b2_index_gather(b2_index* idx, const int64_t* ids, int64_t m, void* out, int
     DeviceGuard guard(idx->device);
     cudaStream_t st = idx->stream;
     const size_t row_bytes = (size_t)idx->d * esize(idx->dtype);
+    if (idx->host && !out_on_device) {  // host rows to host memory: threaded copies, no device work
+        for (int64_t i = 0; i < m; ++i) {
+            if (ids[i] < 0 || ids[i] >= idx->n) { set_error("ids contains a position outside [0, %lld)", (long long)idx->n); return B2_ERANGE; }
+        }
+        const char* src = reinterpret_cast<const char*>(idx->host->main.rows.p);
+        for_each_chunk(m, [&](int64_t lo, int64_t hi) {
+            for (int64_t i = lo; i < hi; ++i) memcpy(reinterpret_cast<char*>(out) + (size_t)i * row_bytes, src + (size_t)ids[i] * row_bytes, row_bytes);
+        });
+        return B2_OK;
+    }
     const int64_t* ids_dev = ids;
     void* out_dev = out;
     if (!out_on_device) {
@@ -714,7 +1138,7 @@ int b2_index_gather(b2_index* idx, const int64_t* ids, int64_t m, void* out, int
         B2_TRY(idx->sub_store.ensure((size_t)m * row_bytes));
         out_dev = idx->sub_store.p;
     }
-    B2_TRY(gather_rows_checked(idx->store.p, idx->dtype, idx->d, ids_dev, m, idx->n, out_dev, idx->scalar, st));
+    B2_TRY(gather_rows_checked(idx->view.store, idx->dtype, idx->d, ids_dev, m, idx->n, out_dev, idx->scalar, st));
     if (!out_on_device) {
         B2_CUDA(cudaMemcpyAsync(out, out_dev, (size_t)m * row_bytes, cudaMemcpyDeviceToHost, st));
         B2_CUDA(cudaStreamSynchronize(st));
@@ -782,6 +1206,43 @@ int b2_debug_filter_lists(b2_index* idx, const void* q, int64_t nq, int32_t q_dt
     const bool lists = cand_score && cand_id && cand_thr;
     DeviceGuard guard(idx->device);
     cudaStream_t st = idx->stream;
+    if (idx->host) {
+        // a host-resident index: the folded lists after the last corpus chunk, the one list of `cap` entries finalize reads,
+        // reported as one split of two halves of cap / 2 (kp = cap) with its bound in both thr entries
+        if (top1) { set_error("the k-means assignment is not available on a host-resident index"); return B2_EINVAL; }
+        HostRows& H = idx->host->main;
+        const void* q_dev = nullptr;
+        if (lists) {
+            B2_TRY(idx->q_in.ensure((size_t)nq * idx->d * esize(q_dtype)));
+            B2_CUDA(cudaMemcpyAsync(idx->q_in.p, q, (size_t)nq * idx->d * esize(q_dtype), cudaMemcpyHostToDevice, st));
+            q_dev = idx->q_in.p;
+            B2_TRY(adapt_queries(idx, q_dev, q_dtype, nq, st));
+        }
+        FilterPlan p;
+        B2_TRY(host_plan(idx, H, q_dev, q_dtype, nq, k, level, p));
+        const int cap = p.use_filter ? finalize_capacity(p.kp, k) : 0;
+        const FilterChunk c = p.use_filter ? p.chunks[0] : FilterChunk();
+        plan[0] = cap ? 1 : 0;
+        plan[1] = cap;
+        plan[2] = 1;
+        plan[3] = 0;
+        plan[4] = c.cluster;
+        plan[5] = p.two_level ? 1 : 0;
+        plan[6] = p.X.filt_dtype;
+        plan[7] = (int32_t)p.chunks.size();
+        *rel_eps = p.rel_eps;
+        if (p.chunks.size() > 1) { set_error("%lld queries take %zu query chunks; one is supported", (long long)nq, p.chunks.size()); return B2_ERANGE; }
+        if (!lists || !cap) return B2_OK;
+        B2_TRY(stream_filter_fold(idx, H, p, c, idx->metric, cap, st));
+        HostStore& hs = *idx->host;
+        B2_CUDA(cudaMemcpyAsync(cand_score, hs.run_score.p, (size_t)nq * cap * sizeof(float), cudaMemcpyDeviceToHost, st));
+        B2_CUDA(cudaMemcpyAsync(cand_id, hs.run_id.p, (size_t)nq * cap * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+        B2_CUDA(cudaMemcpy2DAsync(cand_thr, 2 * sizeof(float), hs.run_thr.p, sizeof(float), sizeof(float), (size_t)nq, cudaMemcpyDeviceToHost, st));
+        B2_CUDA(cudaMemcpy2DAsync(cand_thr + 1, 2 * sizeof(float), hs.run_thr.p, sizeof(float), sizeof(float), (size_t)nq, cudaMemcpyDeviceToHost, st));
+        cudaError_t e = cudaStreamSynchronize(st);
+        if (e != cudaSuccess) { set_error("streamed filter failed on the device: %s", cudaGetErrorString(e)); return B2_ECUDA; }
+        return B2_OK;
+    }
     MatView X = idx->view;
     if (level == 1 || top1) X.filt16 = nullptr;  // the second level drops the bf16 copy; the k-means centroid view has none
     const size_t qbytes = (size_t)nq * idx->d * esize(q_dtype);
@@ -817,6 +1278,29 @@ int b2_debug_filter_lists(b2_index* idx, const void* q, int64_t nq, int32_t q_dt
     B2_CUDA(cudaMemcpyAsync(cand_thr, idx->cand_thr.p, (size_t)nq * c.n_splits * 2 * sizeof(float), cudaMemcpyDeviceToHost, st));
     cudaError_t e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) { set_error("filter failed on the device: %s", cudaGetErrorString(e)); return B2_ECUDA; }
+    return B2_OK;
+}
+
+// The chunking of a host-resident index (no device work): rows per chunk, chunks, ring slots.
+int b2_debug_stream_plan(int64_t n, int32_t d, int32_t dtype, int64_t ring_bytes, int64_t* chunk_rows, int64_t* n_chunks, int32_t* slots) {
+    if (n < 0 || d <= 0 || !dtype_valid(dtype) || ring_bytes < 0 || !chunk_rows || !n_chunks || !slots) { set_error("bad arguments"); return B2_EINVAL; }
+    int nc = 0;
+    B2_TRY(stream_plan(n, d, dtype, (size_t)ring_bytes, chunk_rows, &nc));
+    *n_chunks = nc;
+    *slots = HostStore::SLOTS;
+    return B2_OK;
+}
+
+// Event times of the last search of a host-resident index: [0] copies (copy stream), [1] the span from the first copy to the
+// last fold on the search stream, [2] the filter launches, [3] finalize. Sums over query chunks and levels.
+int b2_debug_stream_times(const b2_index* idx, float* out4) {
+    if (!idx || !out4) { set_error("bad arguments"); return B2_EINVAL; }
+    if (!idx->host) { set_error("not a host-resident index"); return B2_EINVAL; }
+    const HostStore& hs = *idx->host;
+    out4[0] = hs.copy_ms;
+    out4[1] = hs.span_ms;
+    out4[2] = hs.filter_ms;
+    out4[3] = hs.finalize_ms;
     return B2_OK;
 }
 

@@ -17,7 +17,8 @@ namespace b2 {
 // ---- error plumbing ------------------------------------------------------------------------------------
 void set_error(const char* fmt, ...);
 extern int64_t g_stats[8];
-enum { ST_LAUNCHES = 0, ST_QUERIES = 1, ST_FALLBACK = 2, ST_FILTER_LAUNCHES = 3, ST_RESCORED = 4, ST_SECOND_LEVEL = 5 };
+enum { ST_LAUNCHES = 0, ST_QUERIES = 1, ST_FALLBACK = 2, ST_FILTER_LAUNCHES = 3, ST_RESCORED = 4, ST_SECOND_LEVEL = 5,
+       ST_STREAM_BYTES = 6, ST_STREAM_CHUNKS = 7 };
 
 #define B2_CUDA(expr)                                                                              \
     do {                                                                                           \
@@ -185,6 +186,11 @@ int launch_finalize(const MatView& X, const void* q, int q_dtype, int64_t nq, in
                     int n_lists, const float* cand_score, const int32_t* cand_id, const float* cand_thr,
                     float rel_eps, float abs_eps, float q_norm_limit, const int64_t* id_map, int64_t id_offset, float* out_scores,
                     int64_t* out_idx, int32_t* flags, int32_t* sel, int32_t* sel_count, cudaStream_t stream, const float* hint = nullptr);
+int finalize_capacity(int kp, int k);  // candidates finalize keeps through its merge (32 * 2^i), 0 = beyond it
+// host-resident indexes: fold one corpus chunk's lists [nq, n_lists, list_len] (local ids; those below own_lo skipped) into
+// running lists [nq, cap] (global ids = base + local, sorted best first) and their bound [nq]
+int launch_fold_lists(const float* cand_score, const int32_t* cand_id, const float* cand_thr, int64_t nq, int n_lists, int list_len,
+                      int64_t base, int64_t own_lo, int cap, float* run_score, int32_t* run_id, float* run_thr, cudaStream_t stream);
 int shard_lower_bound_max_entries();
 int launch_shard_lower_bound(const float* cand_score, const int32_t* cand_id, int64_t nq, int n_lists, int list_len, int j, const float* qnorm2,
                              float max_norm, float rel_eps, float abs_eps, float q_norm_limit, int metric, float* lower, cudaStream_t stream);

@@ -97,6 +97,7 @@ extern "C" {
 int b2_threshold_pairs(b2_index* idx, float threshold, int32_t part, int32_t nparts, int64_t* out_i, int64_t* out_j, int64_t cap,
                        int64_t* n_pairs) {
     if (!idx) { set_error("Index not loaded"); return B2_EINVAL; }
+    B2_TRY(refuse_host_resident(idx, "b2_threshold_pairs"));
     if (!n_pairs || cap < 0 || (cap > 0 && (!out_i || !out_j))) { set_error("bad output buffers"); return B2_EINVAL; }
     if (nparts <= 0 || part < 0 || part >= nparts) { set_error("bad part/nparts %d/%d", part, nparts); return B2_EINVAL; }
     if (idx->metric != B2_METRIC_IP) { set_error("threshold_pairs is defined for inner-product indexes (sem_dedup thresholds a similarity)"); return B2_EINVAL; }

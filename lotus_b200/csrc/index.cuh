@@ -88,6 +88,68 @@ struct DeviceGuard {
     }
 };
 
+// Pinned, mapped host memory (cudaHostAllocMapped): the device reads it through `dev` (UVA), the copy engines stream from it.
+struct PinnedBuf {
+    void* p = nullptr;
+    void* dev = nullptr;
+    size_t cap = 0;
+    PinnedBuf() = default;
+    PinnedBuf(const PinnedBuf&) = delete;
+    PinnedBuf& operator=(const PinnedBuf&) = delete;
+    ~PinnedBuf() { release(); }
+    int ensure(size_t bytes) {
+        if (bytes <= cap) return B2_OK;
+        release();
+        cudaError_t e = cudaHostAlloc(&p, bytes, cudaHostAllocMapped | cudaHostAllocPortable);
+        if (e == cudaSuccess) e = cudaHostGetDevicePointer(&dev, p, 0);
+        if (e != cudaSuccess) {
+            cudaGetLastError();
+            if (p) cudaFreeHost(p);
+            p = dev = nullptr;
+            set_error("pinning %zu bytes of host memory failed: %s", bytes, cudaGetErrorString(e));
+            return B2_ENOMEM;
+        }
+        cap = bytes;
+        return B2_OK;
+    }
+    void release() {
+        if (p) cudaFreeHost(p);
+        p = dev = nullptr;
+        cap = 0;
+    }
+};
+
+// Rows in pinned host memory plus what a streamed search needs of them on the device: norms, a bf16 copy for the first level of
+// an fp32 store, and the stream plan (host_resident.cu). Used for a host-resident index and for its large ids subsets.
+struct HostRows {
+    PinnedBuf rows;    // [n, d] in dtype, pitch d (what finalize, the dense path and gather read through UVA)
+    PinnedBuf rows16;  // fp32 stores with n >= 4096: the bf16 rounding of the rows (first level), pitch d
+    DevBuf norm2;      // [n] fp32 norms (+ [n] exact int32 norms of an int8 store), the max norm in `scalar`
+    DevBuf scalar;
+    int64_t n = 0;
+    int32_t d = 0, dtype = B2_F32;
+    float max_norm = 0.f;
+    int64_t chunk_rows = 0;  // rows per chunk (multiple of 256 unless one chunk holds every row)
+    int n_chunks = 0;
+};
+
+// The streamed-row machinery of a host-resident index: its rows, the ring of device slots and the copy stream.
+struct HostStore {
+    static constexpr int SLOTS = 2;
+    HostRows main;
+    std::unique_ptr<HostRows> sub;  // an ids subset larger than the ring, gathered on the host
+    size_t ring_bytes = 0;
+    DevBuf slot[SLOTS], slot16[SLOTS];  // streamed rows as the filter reads them; int8 stores: their fp16 form for float queries
+    DevBuf run_score, run_id, run_thr;  // running per-query lists of the fold
+    PinnedBuf staging_ids;
+    cudaStream_t copy = nullptr;
+    cudaEvent_t copied[SLOTS] = {}, freed[SLOTS] = {};
+    std::vector<cudaEvent_t> ev;  // timing: per chunk copy start / end (copy stream), filter start / end (search stream)
+    cudaEvent_t span0 = nullptr, span1 = nullptr, fin0 = nullptr, fin1 = nullptr;
+    float copy_ms = 0.f, span_ms = 0.f, filter_ms = 0.f, finalize_ms = 0.f;  // last search
+    ~HostStore();
+};
+
 // One run of the top-k filter over a view, decided in one place (plan_filter) for every caller: the plain search, the staged
 // sharded search, the k-means assignment and b2_debug_filter_plan.
 struct FilterChunk {  // the queries [q0, q0 + nq) of the call, filtered by one launch
@@ -150,10 +212,22 @@ struct b2_index {
     DevBuf q_norm2;
     DevBuf q_wide;  // int8 queries on a floating-point store, widened exactly
     b2_index* f16_twin = nullptr;  // int8 indexes: the fp16 copy k-means runs on (kmeans_view)
+    // host-resident indexes (b2_index_create_host): the rows live in pinned, mapped host memory and searches stream them
+    // through a ring of device slots (host_resident.cu); `store` stays empty and `view.store` is the mapped pointer
+    std::unique_ptr<b2::HostStore> host;
     ~b2_index();  // destroys the stream and events; the buffers free themselves
 };
 
 namespace b2 {
+
+// B2_EINVAL for the operations a host-resident index does not offer (dedup, k-means, the staged / packed sharded search)
+inline int refuse_host_resident(const b2_index* idx, const char* what) {
+    if (idx && idx->host) {
+        set_error("%s is not available on a host-resident index", what);
+        return B2_EINVAL;
+    }
+    return B2_OK;
+}
 
 // searchable view (filter operand, row norms, max norm) of a row-major device matrix
 int build_view(const void* store, int64_t n, int d, int dtype, DevBuf& filt_pad, DevBuf& norm2, DevBuf& scalar, MatView& v,

@@ -1003,6 +1003,7 @@ extern "C" {
 int b2_kmeans(b2_index* idx, const int64_t* ids, int64_t m, int32_t k, int32_t niter, int64_t seed, int32_t full_lloyd,
               int64_t* out_assign, float* out_centroids, float* out_obj) {
     if (!idx) { set_error("Index not loaded"); return B2_EINVAL; }
+    B2_TRY(refuse_host_resident(idx, "k-means"));
     {
         DeviceGuard twin_guard(idx->device);
         B2_TRY(kmeans_view(idx, &idx));
@@ -1025,6 +1026,7 @@ int b2_kmeans(b2_index* idx, const int64_t* ids, int64_t m, int32_t k, int32_t n
 int b2_kmeans_assign_dev(b2_index* idx, const int64_t* ids_dev, int64_t m, const float* centroids_dev, int32_t k, int64_t* assign_dev,
                          float* dist_dev, void* stream) {
     if (!idx) { set_error("Index not loaded"); return B2_EINVAL; }
+    B2_TRY(refuse_host_resident(idx, "k-means"));
     {
         DeviceGuard twin_guard(idx->device);
         B2_TRY(kmeans_view(idx, &idx));
@@ -1047,6 +1049,7 @@ int b2_kmeans_assign_dev(b2_index* idx, const int64_t* ids_dev, int64_t m, const
 int b2_kmeans_accumulate_dev(b2_index* idx, const int64_t* ids_dev, int64_t m, const int64_t* assign_dev, int32_t k,
                              const float* centroids_dev, float* sums_dev, float* counts_dev, double* obj_dev, void* stream) {
     if (!idx) { set_error("Index not loaded"); return B2_EINVAL; }
+    B2_TRY(refuse_host_resident(idx, "k-means"));
     {
         DeviceGuard twin_guard(idx->device);
         B2_TRY(kmeans_view(idx, &idx));
@@ -1067,6 +1070,7 @@ int b2_kmeans_accumulate_dev(b2_index* idx, const int64_t* ids_dev, int64_t m, c
 int b2_kmeans_accumulate(b2_index* idx, const int64_t* ids, int64_t m, const int64_t* assign, int32_t k, float* out_sums,
                          float* out_counts) {
     if (!idx) { set_error("Index not loaded"); return B2_EINVAL; }
+    B2_TRY(refuse_host_resident(idx, "k-means"));
     {
         DeviceGuard twin_guard(idx->device);
         B2_TRY(kmeans_view(idx, &idx));
@@ -1103,6 +1107,7 @@ int b2_kmeans_accumulate(b2_index* idx, const int64_t* ids, int64_t m, const int
 int b2_kmeans_assign(b2_index* idx, const int64_t* ids, int64_t m, const float* centroids, int32_t k, int64_t* out_assign,
                      float* out_dist) {
     if (!idx) { set_error("Index not loaded"); return B2_EINVAL; }
+    B2_TRY(refuse_host_resident(idx, "k-means"));
     {
         DeviceGuard twin_guard(idx->device);
         B2_TRY(kmeans_view(idx, &idx));

@@ -553,6 +553,64 @@ __global__ void __launch_bounds__(FIN_WARPS * 32) finalize_kernel(const Finalize
 template <int R>
 __global__ void __launch_bounds__(FIN_WARPS * 32) finalize_i8_kernel(const FinalizeParams p) { finalize_body<R, true>(p); }
 
+// ---- fold of one corpus chunk's candidate lists into running lists (host-resident indexes) -----------------------------
+// Per query (one warp): the running list (32*R entries, sorted best first by filter score, id -1 = empty) absorbs the chunk's
+// n_lists lists of list_len entries. Chunk ids are made global (base + local); entries whose local id is below own_lo (rows an
+// earlier chunk already covered, where the last chunk overlaps its predecessor) are skipped. The running bound becomes the
+// maximum of itself, the chunk's bounds and the best filter score the merge dropped, exactly as finalize's own merge forms it,
+// so the two certificate premises hold for every row folded so far (DESIGN.md §2).
+template <int R>
+__global__ void __launch_bounds__(128) fold_lists_kernel(const float* cand_score, const int32_t* cand_id, const float* cand_thr,
+                                                         int64_t nq, int n_lists, int list_len, int32_t base, int32_t own_lo,
+                                                         float* run_score, int32_t* run_id, float* run_thr) {
+    constexpr int NC = 32 * R;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int64_t q = blockIdx.x * 4ll + warp;
+    if (q >= nq) return;
+    uint64_t keys[R];
+#pragma unroll
+    for (int r = 0; r < R; ++r) {
+        const size_t off = (size_t)q * NC + r * 32 + lane;
+        const int32_t id = run_id[off];
+        keys[r] = id >= 0 ? ((uint64_t)(~f32_ord(run_score[off])) << 32) | (uint32_t)id : KEY_WORST;
+    }
+    float bound = lane == 0 ? run_thr[q] : -INFINITY;
+    const int lists_per_chunk = max(1, NC / list_len);
+    const size_t qbase = (size_t)q * n_lists;
+    for (int s0 = 0; s0 < n_lists; s0 += lists_per_chunk) {
+        uint64_t chunk[R];
+        bool any_key = false;
+#pragma unroll
+        for (int r = 0; r < R; ++r) {
+            const int e = r * 32 + lane;
+            const int li = e / list_len, pos = e - li * list_len;
+            uint64_t kk = KEY_WORST;
+            if (li < lists_per_chunk && s0 + li < n_lists) {
+                const size_t off = (qbase + s0 + li) * list_len + pos;
+                const int32_t id = cand_id[off];
+                if (id >= own_lo) kk = ((uint64_t)(~f32_ord(cand_score[off])) << 32) | (uint32_t)(id + base);
+            }
+            chunk[r] = kk;
+            any_key |= kk != KEY_WORST;
+        }
+        for (int li = lane; li < lists_per_chunk && s0 + li < n_lists; li += 32) bound = fmaxf(bound, cand_thr[qbase + s0 + li]);
+        if (!__any_sync(FULL, any_key)) continue;
+        warp_bitonic_sort<R>(chunk, lane);
+        const uint64_t drop = warp_merge_keep_low<R>(keys, chunk, lane);
+        if (drop != KEY_WORST) bound = fmaxf(bound, f32_unord(~(uint32_t)(drop >> 32)));
+    }
+#pragma unroll
+    for (int off = 16; off >= 1; off >>= 1) bound = fmaxf(bound, __shfl_xor_sync(FULL, bound, off));
+#pragma unroll
+    for (int r = 0; r < R; ++r) {
+        const size_t off = (size_t)q * NC + r * 32 + lane;
+        const bool v = keys[r] != KEY_WORST;
+        run_score[off] = v ? f32_unord(~(uint32_t)(keys[r] >> 32)) : -INFINITY;
+        run_id[off] = v ? (int32_t)(uint32_t)(keys[r] & 0xffffffffu) : -1;
+    }
+    if (lane == 0) run_thr[q] = bound;
+}
+
 // ---- dense exact path -----------------------------------------------------------------------------------------
 // scores[s, j] = canonical score of selected query s against row j. One warp per row; the row's share stays
 // in registers/L1 while the warp walks the selected queries.
@@ -1053,17 +1111,52 @@ int launch_finalize(const MatView& X, const void* q, int q_dtype, int64_t nq, in
     p.max_norm = X.max_norm;
     p.max_norm_dev = X.max_norm_dev;
     g_stats[ST_RESCORED] += nq * (int64_t)kp;
-    // survivors kept through the merge: the filter's list capacity for k <= 64; k + 32 when several splits share a large k
-    // (the 32 extra by-filter-score candidates are what the prune / certificate margins need)
-    const int need = std::max(kp, k > 64 ? std::min(k + 32, 1024) : 0);
-    if (need <= 32) return launch_finalize_r<1>(p, stream);
-    if (need <= 64) return launch_finalize_r<2>(p, stream);
-    if (need <= 128) return launch_finalize_r<4>(p, stream);
-    if (need <= 256) return launch_finalize_r<8>(p, stream);
-    if (need <= 512) return launch_finalize_r<16>(p, stream);
-    if (need <= 1024) return launch_finalize_r<32>(p, stream);
-    set_error("internal: finalize capacity %d", need);
+    switch (finalize_capacity(kp, k)) {
+        case 32: return launch_finalize_r<1>(p, stream);
+        case 64: return launch_finalize_r<2>(p, stream);
+        case 128: return launch_finalize_r<4>(p, stream);
+        case 256: return launch_finalize_r<8>(p, stream);
+        case 512: return launch_finalize_r<16>(p, stream);
+        case 1024: return launch_finalize_r<32>(p, stream);
+    }
+    set_error("internal: finalize capacity for kp=%d k=%d", kp, k);
     return B2_EINVAL;
+}
+
+// survivors kept through the merge: the filter's list capacity for k <= 64; k + 32 when several splits share a large k
+// (the 32 extra by-filter-score candidates are what the prune / certificate margins need), rounded up to 32 * 2^i
+int finalize_capacity(int kp, int k) {
+    const int need = std::max(kp, k > 64 ? std::min(k + 32, 1024) : 0);
+    int cap = 32;
+    while (cap < need && cap < 1024) cap <<= 1;
+    return need <= cap ? cap : 0;
+}
+
+template <int R>
+static void launch_fold_r(const float* cs, const int32_t* ci, const float* ct, int64_t nq, int n_lists, int list_len, int32_t base,
+                          int32_t own_lo, float* rs, int32_t* ri, float* rt, cudaStream_t stream) {
+    fold_lists_kernel<R><<<(unsigned)ceil_div(nq, 4), 128, 0, stream>>>(cs, ci, ct, nq, n_lists, list_len, base, own_lo, rs, ri, rt);
+}
+
+int launch_fold_lists(const float* cand_score, const int32_t* cand_id, const float* cand_thr, int64_t nq, int n_lists, int list_len,
+                      int64_t base, int64_t own_lo, int cap, float* run_score, int32_t* run_id, float* run_thr, cudaStream_t stream) {
+    if (nq <= 0) return B2_OK;
+    if (list_len > cap || base + own_lo > 0x7fffffffLL) {
+        set_error("internal: fold of lists of %d into %d entries at row %lld", list_len, cap, (long long)base);
+        return B2_EINVAL;
+    }
+    const int32_t b = (int32_t)base, o = (int32_t)own_lo;
+    switch (cap) {
+        case 32: launch_fold_r<1>(cand_score, cand_id, cand_thr, nq, n_lists, list_len, b, o, run_score, run_id, run_thr, stream); break;
+        case 64: launch_fold_r<2>(cand_score, cand_id, cand_thr, nq, n_lists, list_len, b, o, run_score, run_id, run_thr, stream); break;
+        case 128: launch_fold_r<4>(cand_score, cand_id, cand_thr, nq, n_lists, list_len, b, o, run_score, run_id, run_thr, stream); break;
+        case 256: launch_fold_r<8>(cand_score, cand_id, cand_thr, nq, n_lists, list_len, b, o, run_score, run_id, run_thr, stream); break;
+        case 512: launch_fold_r<16>(cand_score, cand_id, cand_thr, nq, n_lists, list_len, b, o, run_score, run_id, run_thr, stream); break;
+        case 1024: launch_fold_r<32>(cand_score, cand_id, cand_thr, nq, n_lists, list_len, b, o, run_score, run_id, run_thr, stream); break;
+        default: set_error("internal: fold capacity %d", cap); return B2_EINVAL;
+    }
+    B2_LAUNCH_CHECK();
+    return B2_OK;
 }
 
 // workspace bytes the full-sort path needs for `rows` score rows of length n: keys in + keys out + the sort's scratch

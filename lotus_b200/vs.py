@@ -253,6 +253,28 @@ def merge_shard_lists(D_parts: list, I_parts: list, metric: int):
     return np.take_along_axis(D, sel, axis=1), np.take_along_axis(I, sel, axis=1)
 
 
+def _free_device_bytes(device: int) -> int:
+    """Free memory of a device in bytes (cudaMemGetInfo)."""
+    import torch
+    return int(torch.cuda.mem_get_info(device)[0])
+
+
+def device_footprint(n: int, d: int, code: int) -> int:
+    """Device bytes of a device-resident index of n x d rows of element type `code`: the rows, their padded copy when a row is
+    not a multiple of 16 bytes, the bf16 copy of an fp32 store of at least 4096 rows, and the norms."""
+    esz = {nv.F32: 4, nv.BF16: 2, nv.F16: 2, nv.I8: 1}[code]
+    align = 16 // esz
+    total = n * d * esz
+    if d % align:
+        total += n * (-(-d // align) * align) * esz
+    if code == nv.F32 and n >= 4096:
+        total += n * (-(-d // 8) * 8) * 2
+    return total + n * (8 if code == nv.I8 else 4)
+
+
+AUTO_MARGIN = 1 << 30  # residency="auto": device memory left free beyond the footprint, for search workspaces
+
+
 class B200VS(VS):
     """Flat (brute-force, exact) vector store on one H100 (or, with devices=[...], row-sharded over several from one process).
 
@@ -265,13 +287,25 @@ class B200VS(VS):
     are searched on the int8 tensor cores, floating-point queries against an fp16 copy of the rows made on their first
     search; results equal faiss on the float32 upcast; dedup and k-means are not available), or "auto" (bf16 only when
     handed a bf16 tensor, float32 otherwise; int8 input still gives a float32 store).
+    residency: "device" (default: the rows live in device memory), "host" (the rows stay in pinned host memory and every
+    search streams them through a device ring of ring_bytes, None = the library default: corpora larger than free device
+    memory, same results bit for bit; threshold_pairs / kmeans, hence sem_dedup / sem_cluster_by, raise ValueError) or
+    "auto" (device when the store's device footprint plus a 1 GiB margin fits in free device memory, host otherwise;
+    `resident(index_dir)` reports the choice). CUDA tensors given to a host-resident store are copied to the host.
     """
 
     accepts_id_arrays = True  # `ids=` may be a numpy int64 array (the operators then skip building a Python list)
 
     def __init__(self, factory_string: str = "Flat", metric: int = METRIC_INNER_PRODUCT, dtype: str = "auto",
-                 device: int = 0, cache_size: int = 4, devices: "list[int] | None" = None):
+                 device: int = 0, cache_size: int = 4, devices: "list[int] | None" = None, residency: str = "device",
+                 ring_bytes: "int | None" = None):
         super().__init__()
+        if residency not in ("device", "host", "auto"):
+            raise ValueError("residency must be 'device', 'host' or 'auto'")
+        if ring_bytes is not None and (not isinstance(ring_bytes, int) or ring_bytes < 0):
+            raise ValueError("ring_bytes must be a non-negative int or None")
+        if devices and len(devices) > 1 and residency == "host":
+            raise ValueError("residency='host' serves one device; it cannot be combined with devices=[...]")
         if factory_string != "Flat":
             raise ValueError(f"B200VS implements the flat (exact) index only; factory_string={factory_string!r}")
         if metric not in (METRIC_INNER_PRODUCT, METRIC_L2):
@@ -289,6 +323,20 @@ class B200VS(VS):
         self._cache: "OrderedDict[str, tuple[float, nv.Index, Any]]" = OrderedDict()
         self._cache_size = max(2, cache_size)
         self._scratch: dict = {}
+        self.residency = residency
+        self.ring_bytes = ring_bytes
+
+    def _choose_residency(self, n: int, d: int, code: int) -> str:
+        if self.residency != "auto":
+            return self.residency
+        return "device" if device_footprint(n, d, code) + AUTO_MARGIN <= _free_device_bytes(self.device) else "host"
+
+    def resident(self, index_dir: "str | None" = None) -> str:
+        """Where the rows of the loaded index (or of the cached index of `index_dir`) live: "device" or "host"."""
+        idx = self.b2_index if index_dir is None else self._cache[os.path.abspath(index_dir)][1]
+        if idx is None:
+            raise ValueError("Index not loaded")
+        return getattr(idx, "resident", "device")
 
     # -- index lifetime ---------------------------------------------------------------------------------------------
     def _build(self, embeddings: Any) -> nv.Index:
@@ -301,6 +349,11 @@ class B200VS(VS):
                 want16 = want16 or (self.dtype == "auto" and t.dtype == torch.bfloat16)
             host, code, _ = _to_host_matrix(embeddings, want16, want_f16=self.dtype == "f16", want_i8=self.dtype == "i8")
             return MultiDeviceIndex(host, code, self.metric, self.devices)  # type: ignore[return-value]
+        if self.residency != "device":
+            want16 = self.dtype == "bf16" or (self.dtype == "auto" and t is not None and str(t.dtype) == "torch.bfloat16")
+            host, code, _ = _to_host_matrix(embeddings, want16, want_f16=self.dtype == "f16", want_i8=self.dtype == "i8")
+            where = self._choose_residency(host.shape[0], host.shape[1], code)
+            return nv.Index(host, code, self.metric, self.device, residency=where, ring_bytes=self.ring_bytes or 0)
         if t is not None and t.dim() == 2 and t.device.index == self.device:
             # device hand-off: the encoder's output never visits the host on its way into the index (a tensor that
             # already has the store's type is read in place)
@@ -442,14 +495,21 @@ class B200VS(VS):
         return RMOutput(distances=out_s.cpu().numpy(), indices=out_i.cpu().numpy())
 
     # -- extensions used by the re-registered operators --------------------------------------------------------------
+    def _refuse_host(self, what: str) -> None:
+        if getattr(self.b2_index, "resident", "device") == "host":
+            raise ValueError(f"{what} is not available on a host-resident index (B200VS(residency='host')): build the store "
+                             "with residency='device'")
+
     def threshold_pairs(self, threshold: float):
         if self.b2_index is None:
             raise ValueError("Index not loaded")
+        self._refuse_host("threshold_pairs (sem_dedup)")
         return self.b2_index.threshold_pairs(threshold)
 
     def kmeans(self, ids: Any, ncentroids: int, niter: int = 20, seed: int = 1234, full_lloyd: bool = False):
         if self.b2_index is None:
             raise ValueError("Index not loaded")
+        self._refuse_host("kmeans (sem_cluster_by)")
         return self.b2_index.kmeans(ncentroids, niter=niter, seed=seed, ids=np.asarray(ids, dtype=np.int64), full_lloyd=full_lloyd)
 
     def close(self) -> None:
