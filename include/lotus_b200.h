@@ -163,6 +163,17 @@ B2_API int b2_index_search_stage1_dev(b2_index* idx, const void* q_dev, int64_t 
                                float* lower_dev, void* stream);
 B2_API int b2_index_search_stage2_packed_dev(b2_index* idx, const float* hint_dev, uint64_t* out_packed_dev, void* stream);
 
+/* ---- range search (faiss IndexFlat.range_search) ------------------------------------------------------ */
+/* Every row whose canonical score is strictly greater than `radius` (B2_METRIC_IP), or whose canonical squared distance is
+ * strictly less than it (B2_METRIC_L2), for each query q[nq,d] in q_dtype. HOST buffers, in the layout of faiss's Python
+ * range_search: lims[nq+1] int64; out_d / out_i [lims[nq]] hold query i's hits at [lims[i], lims[i+1]), in ascending row id,
+ * with the same canonical float32 values b2_index_search reports. ids != NULL: only those rows (positions into the index, any
+ * order, repeats allowed), as a temporary index over x[ids]: a query's hits follow the order of `ids` and report the original
+ * ids. A NaN radius matches nothing. lims and *n_results are filled on success and also when the call returns B2_ERANGE
+ * because cap < *n_results; the caller then retries with cap = *n_results. Every index residency and dtype. */
+B2_API int b2_index_range_search(b2_index* idx, const void* q, int64_t nq, int32_t q_dtype, float radius, const int64_t* ids,
+                                 int64_t n_ids, int64_t* lims, float* out_d, int64_t* out_i, int64_t cap, int64_t* n_results);
+
 /* ---- row gather (faiss_vs.py:38-41) ------------------------------------------------------------------ */
 /* out[m,d] in the index's dtype = x[ids]; HOST out unless out_on_device != 0 (then ids is a device pointer too) */
 B2_API int b2_index_gather(b2_index* idx, const int64_t* ids, int64_t m, void* out, int32_t out_on_device);
@@ -250,6 +261,9 @@ B2_API int b2_debug_stream_times(const b2_index* idx, float* out4);
  * B2_BF16 / B2_F16 = 2-byte wgmma) with queries of `q_dtype`, dimension d. abs_eps is non-zero only where an operand is
  * rounded to fp16 (its subnormal spacing). For testing; the search paths use the same function. */
 B2_API int b2_debug_filter_eps(int32_t store_dtype, int32_t filt_dtype, int32_t q_dtype, int32_t d, float* rel_eps, float* abs_eps);
+/* The last b2_index_range_search of this handle: out4[0] the most candidates one range-filter launch produced (the peak size
+ * of the candidate buffer), [1] the hits, [2] the queries the exact dense path answered, [3] 1 if the filter ran. */
+B2_API int b2_debug_range_stats(const b2_index* idx, int64_t* out4);
 
 /* ---- instrumentation ---------------------------------------------------------------------------------- */
 /* counters since the last b2_stats_reset(): [0] kernels launched by this library, [1] queries answered,

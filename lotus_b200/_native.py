@@ -24,7 +24,7 @@ SYMBOLS = [
     "b2_index_search", "b2_index_search_dev", "b2_merge_topk_dev", "b2_index_search_packed_dev", "b2_merge_topk_packed_dev", "b2_index_search_stage1_dev", "b2_index_search_stage2_packed_dev", "b2_index_gather", "b2_threshold_pairs",
     "b2_connected_components", "b2_kmeans", "b2_kmeans_assign", "b2_kmeans_accumulate", "b2_kmeans_assign_dev", "b2_kmeans_accumulate_dev", "b2_stats", "b2_stats_reset", "b2_last_filter_ms", "b2_host_f32_to_bf16", "b2_host_bf16_to_f32", "b2_debug_filter_plan",
     "b2_debug_filter_lists", "b2_debug_filter_eps", "b2_index_create_host", "b2_index_resident", "b2_debug_stream_plan",
-    "b2_debug_stream_times",
+    "b2_debug_stream_times", "b2_index_range_search", "b2_debug_range_stats",
 ]
 
 
@@ -84,6 +84,10 @@ def lib() -> ctypes.CDLL:
     L.b2_index_search_stage1_dev.argtypes = [vp, vp, i64, i32, i32, i32, vp, vp]
     L.b2_index_search_stage2_packed_dev.restype = c.c_int
     L.b2_index_search_stage2_packed_dev.argtypes = [vp, vp, vp, vp]
+    L.b2_index_range_search.restype = c.c_int
+    L.b2_index_range_search.argtypes = [vp, vp, i64, i32, f32, vp, i64, vp, vp, vp, i64, c.POINTER(i64)]
+    L.b2_debug_range_stats.restype = c.c_int
+    L.b2_debug_range_stats.argtypes = [vp, c.POINTER(i64)]
     L.b2_index_gather.restype = c.c_int
     L.b2_index_gather.argtypes = [vp, vp, i64, vp, i32]
     L.b2_threshold_pairs.restype = c.c_int
@@ -303,6 +307,40 @@ class Index:
         check(lib().b2_index_search(self._h, _ptr(q) if nq else None, nq, q_dtype, k, _ptr(ids_a),
                                     0 if ids_a is None else len(ids_a), _ptr(D), _ptr(I)))
         return D, I
+
+    def range_search(self, q: np.ndarray, radius: float, q_dtype: int = F32, ids: Optional[np.ndarray] = None,
+                     cap: Optional[int] = None):
+        """faiss IndexFlat.range_search: (lims[nq+1] int64, D[lims[nq]] float32, I[lims[nq]] int64), query i's hits at
+        [lims[i], lims[i+1]) in ascending row id (with ids: in the order of `ids`, reported as the original ids). IP keeps the
+        rows scoring strictly above `radius`, L2 those strictly closer than it (squared distance). Host buffers; when the
+        result outgrows `cap` the call is repeated once with the exact size."""
+        q = np.ascontiguousarray(q)
+        nq = q.shape[0]
+        if nq and q.shape[1] != self.d:
+            raise ValueError(f"query dimension {q.shape[1]} != index dimension {self.d}")
+        ids_a = None if ids is None else np.ascontiguousarray(ids, dtype=np.int64)
+        lims = np.zeros(nq + 1, dtype=np.int64)
+        cap = int(cap) if cap is not None else max(1 << 16, 64 * nq)
+        for attempt in range(2):
+            D = np.empty(cap, dtype=np.float32)
+            I = np.empty(cap, dtype=np.int64)
+            total = ctypes.c_int64(0)
+            rc = lib().b2_index_range_search(self._h, _ptr(q) if nq else None, nq, q_dtype, float(radius), _ptr(ids_a),
+                                             0 if ids_a is None else len(ids_a), _ptr(lims), _ptr(D), _ptr(I), cap,
+                                             ctypes.byref(total))
+            if rc == ERANGE and attempt == 0 and total.value > cap:
+                cap = int(total.value)
+                continue
+            check(rc)
+            break
+        m = int(total.value)
+        return lims, D[:m].copy(), I[:m].copy()
+
+    def range_stats(self) -> dict:
+        """Counts of the last range_search (b2_debug_range_stats)."""
+        out = (ctypes.c_int64 * 4)()
+        check(lib().b2_debug_range_stats(self._h, out))
+        return {"candidates_peak": out[0], "hits": out[1], "dense_queries": out[2], "filtered": bool(out[3])}
 
     def search_dev(self, q_ptr: int, nq: int, k: int, q_dtype: int, out_scores_ptr: int, out_idx_ptr: int,
                    id_offset: int = 0, ids_ptr: Optional[int] = None, n_ids: int = 0, stream: int = 0) -> None:

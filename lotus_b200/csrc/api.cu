@@ -698,6 +698,8 @@ static int stream_search(b2_index* idx, HostRows& H, int metric, const void* q_d
 // A search of a host-resident index: the whole index, or an ids subset (ids_host and / or ids_dev; ids_dev is what the results
 // map through). A subset whose rows fit in the ring is gathered from host memory into a device view and searched as on a
 // device-resident index; a larger one is gathered on the host, by threads, into pinned staging and streamed.
+static int gather_host_subset(b2_index* idx, const int64_t* ids_host, const int64_t* ids_dev, int64_t n_ids, cudaStream_t st);
+
 static int host_search(b2_index* idx, const void* q_dev, int q_dtype, int64_t nq, int k, const int64_t* ids_host, const int64_t* ids_dev,
                        int64_t n_ids, int64_t id_offset, float* out_sc, int64_t* out_id, cudaStream_t st) {
     HostStore& hs = *idx->host;
@@ -707,6 +709,13 @@ static int host_search(b2_index* idx, const void* q_dev, int q_dtype, int64_t nq
         B2_TRY(build_subset(idx, ids_dev, n_ids, q_dtype, sub, st));
         return search_core(idx, sub, idx->metric, q_dev, q_dtype, nq, k, ids_dev, 0, out_sc, out_id, st);
     }
+    B2_TRY(gather_host_subset(idx, ids_host, ids_dev, n_ids, st));
+    return stream_search(idx, *hs.sub, idx->metric, q_dev, q_dtype, nq, k, ids_dev, 0, out_sc, out_id, st, 0);
+}
+
+// the rows x[ids] of a host-resident index gathered on the host, by threads, into hs.sub (pinned), with their norms and plan
+static int gather_host_subset(b2_index* idx, const int64_t* ids_host, const int64_t* ids_dev, int64_t n_ids, cudaStream_t st) {
+    HostStore& hs = *idx->host;
     if (!ids_host) {
         B2_TRY(hs.staging_ids.ensure((size_t)n_ids * sizeof(int64_t)));
         B2_CUDA(cudaMemcpyAsync(hs.staging_ids.p, ids_dev, (size_t)n_ids * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
@@ -728,8 +737,100 @@ static int host_search(b2_index* idx, const void* q_dev, int q_dtype, int64_t nq
     for_each_chunk(n_ids, [&](int64_t lo, int64_t hi) {
         for (int64_t i = lo; i < hi; ++i) memcpy(dst + (size_t)i * row, src + (size_t)ids_host[i] * row, row);
     });
-    B2_TRY(host_rows_init(S, n_ids, idx->d, idx->dtype, hs.ring_bytes, st));
-    return stream_search(idx, S, idx->metric, q_dev, q_dtype, nq, k, ids_dev, 0, out_sc, out_id, st, 0);
+    return host_rows_init(S, n_ids, idx->d, idx->dtype, hs.ring_bytes, st);
+}
+
+// ---- range search (range.cu) ----------------------------------------------------------------------------------------------
+// The filter operand of a device-resident view: float queries on an int8 store use its fp16 copy (exact). An fp32 store filters
+// with tf32 on its own rows (its bf16 first-level copy is a knn optimisation; a range search would only admit more candidates).
+static MatView range_filter_view(const MatView& X, int q_dtype) {
+    MatView v = X;
+    if (X.dtype == B2_I8 && q_dtype != B2_I8) {
+        v.filt = X.filt_f16;
+        v.filt_pitch = X.filt_f16_pitch;
+        v.filt_dtype = B2_F16;
+    }
+    return v;
+}
+
+static int range_device(b2_index* idx, RangeWork& W, const MatView& X, const void* q_dev, int q_dtype, int64_t nq, float radius,
+                        cudaStream_t st) {
+    B2_TRY(range_begin(idx, W, X, idx->metric, q_dev, q_dtype, nq, radius, st));
+    return range_pass(idx, W, range_filter_view(X, q_dtype), X.d, 0, 0, st);
+}
+
+// The range search of streamed rows H: every chunk is filtered and verified while its slot holds it (the copy of the next chunk
+// runs meanwhile), so verification reads device memory only; the last chunk skips the rows its predecessor covered. An int8
+// store with float queries converts each chunk to fp16 for the filter and verifies against the int8 rows.
+static int range_stream(b2_index* idx, RangeWork& W, HostRows& H, const void* q_dev, int q_dtype, int64_t nq, float radius,
+                        cudaStream_t st) {
+    HostStore& hs = *idx->host;
+    MatView Xc = host_view(H);
+    Xc.n = H.chunk_rows;
+    B2_TRY(range_begin(idx, W, Xc, idx->metric, q_dev, q_dtype, nq, radius, st));
+    if (nq <= 0 || H.n <= 0) return B2_OK;
+    const int d = H.d;
+    const bool via_f16 = H.dtype == B2_I8 && q_dtype != B2_I8;
+    const size_t src_row = (size_t)d * esize(H.dtype);
+    const int64_t pitch = via_f16 ? d : Xc.filt_pitch;  // elements per slot row
+    const size_t slot_pitch = (size_t)pitch * esize(H.dtype);
+    const int64_t f16_pitch = round_up(d, tma_align_elems(B2_F16));
+    const int64_t R = H.chunk_rows;
+    for (int s = 0; s < HostStore::SLOTS; ++s) {
+        B2_TRY(hs.slot[s].ensure((size_t)R * slot_pitch));
+        if (via_f16) B2_TRY(hs.slot16[s].ensure((size_t)R * f16_pitch * 2));
+    }
+    const char* src = reinterpret_cast<const char*>(H.rows.p);
+    auto issue_copy = [&](int ch) -> int {
+        const int s = ch % HostStore::SLOTS;
+        const int64_t base = std::min<int64_t>((int64_t)ch * R, H.n - R);
+        B2_CUDA(cudaStreamWaitEvent(hs.copy, hs.freed[s], 0));  // the slot's previous chunk has been verified
+        B2_CUDA(cudaMemcpy2DAsync(hs.slot[s].p, slot_pitch, src + (size_t)base * src_row, src_row, src_row, (size_t)R,
+                                  cudaMemcpyHostToDevice, hs.copy));
+        B2_CUDA(cudaEventRecord(hs.copied[s], hs.copy));
+        g_stats[ST_STREAM_BYTES] += R * (int64_t)src_row;
+        return B2_OK;
+    };
+    const int nc = H.n_chunks;
+    B2_TRY(issue_copy(0));
+    for (int ch = 0; ch < nc; ++ch) {
+        if (ch + 1 < nc) B2_TRY(issue_copy(ch + 1));
+        const int s = ch % HostStore::SLOTS;
+        const int64_t base = std::min<int64_t>((int64_t)ch * R, H.n - R);
+        B2_CUDA(cudaStreamWaitEvent(st, hs.copied[s], 0));
+        MatView Xs = Xc;
+        Xs.store = hs.slot[s].p;
+        Xs.filt = hs.slot[s].p;
+        Xs.filt_pitch = pitch;
+        Xs.filt_dtype = H.dtype;
+        if (via_f16) {
+            if (W.use_filter) B2_TRY(launch_convert_pad(hs.slot[s].p, B2_I8, R, d, hs.slot16[s].p, B2_F16, f16_pitch, st));
+            Xs.filt = hs.slot16[s].p;
+            Xs.filt_pitch = f16_pitch;
+            Xs.filt_dtype = B2_F16;
+        }
+        Xs.norm2 = Xc.norm2 + base;
+        Xs.norm2_i8 = Xc.norm2_i8 ? Xc.norm2_i8 + base : nullptr;
+        B2_TRY(range_pass(idx, W, Xs, pitch, base, (int64_t)ch * R - base, st));  // synchronises: the slot is free afterwards
+        B2_CUDA(cudaEventRecord(hs.freed[s], st));
+        g_stats[ST_STREAM_CHUNKS]++;
+    }
+    return B2_OK;
+}
+
+// A range search of a host-resident index: the whole index streamed, or an ids subset (gathered into a device view when its rows
+// fit in the ring, else gathered on the host and streamed), as host_search does. *id_map: what the hit positions map through.
+static int host_range(b2_index* idx, RangeWork& W, const void* q_dev, int q_dtype, int64_t nq, float radius, const int64_t* ids_host,
+                      const int64_t* ids_dev, int64_t n_ids, cudaStream_t st) {
+    HostStore& hs = *idx->host;
+    if (!ids_dev) return range_stream(idx, W, hs.main, q_dev, q_dtype, nq, radius, st);
+    if ((size_t)n_ids * ring_row_bytes(idx->d, idx->dtype) <= hs.ring_bytes) {
+        MatView sub;
+        B2_TRY(build_subset(idx, ids_dev, n_ids, q_dtype, sub, st));
+        return range_device(idx, W, sub, q_dev, q_dtype, nq, radius, st);
+    }
+    B2_TRY(gather_host_subset(idx, ids_host, ids_dev, n_ids, st));
+    return range_stream(idx, W, *hs.sub, q_dev, q_dtype, nq, radius, st);
 }
 
 }  // namespace b2
@@ -1005,6 +1106,79 @@ int b2_index_search(b2_index* idx, const void* q, int64_t nq, int32_t q_dtype, i
     B2_CUDA(cudaMemcpyAsync(out_idx, idx->out_id.p, (size_t)nq * k * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
     cudaError_t e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) { set_error("search failed on the device: %s", cudaGetErrorString(e)); return B2_ECUDA; }
+    return B2_OK;
+}
+
+int b2_index_range_search(b2_index* idx, const void* q, int64_t nq, int32_t q_dtype, float radius, const int64_t* ids, int64_t n_ids,
+                          int64_t* lims, float* out_d, int64_t* out_i, int64_t cap, int64_t* n_results) {
+    if (!idx) { set_error("Index not loaded"); return B2_EINVAL; }
+    if (nq < 0 || (nq > 0 && !q)) { set_error("bad query batch"); return B2_EINVAL; }
+    if (!dtype_valid(q_dtype)) { set_error("q_dtype must be B2_F32, B2_BF16, B2_F16 or B2_I8"); return B2_EINVAL; }
+    if (!lims || !n_results) { set_error("lims / n_results are NULL"); return B2_EINVAL; }
+    if (cap < 0 || (cap > 0 && (!out_d || !out_i))) { set_error("bad output buffers (cap=%lld)", (long long)cap); return B2_EINVAL; }
+    if (ids && n_ids < 0) { set_error("n_ids < 0"); return B2_EINVAL; }
+    if (nq > 0x7fffff00LL) { set_error("too many queries for one range search (nq=%lld)", (long long)nq); return B2_ERANGE; }
+    *n_results = 0;
+    if (nq == 0 || radius != radius) {  // a NaN radius: every comparison is false
+        for (int64_t i = 0; i <= nq; ++i) lims[i] = 0;
+        return B2_OK;
+    }
+    DeviceGuard guard(idx->device);
+    cudaStream_t st = idx->stream;
+    if (!idx->range) idx->range.reset(new RangeWork());
+    RangeWork& W = *idx->range;
+    idx->last_filter_ms = -1.f;
+    const size_t qbytes = (size_t)nq * idx->d * esize(q_dtype);
+    B2_TRY(idx->q_in.ensure(qbytes));
+    B2_CUDA(cudaMemcpyAsync(idx->q_in.p, q, qbytes, cudaMemcpyHostToDevice, st));
+    const void* q_dev = idx->q_in.p;
+    B2_TRY(adapt_queries(idx, q_dev, q_dtype, nq, st));
+    const int64_t* ids_dev = nullptr;
+    if (ids) {
+        bool identity = n_ids == idx->n;
+        for (int64_t i = 0; identity && i < n_ids; ++i) identity = ids[i] == i;
+        if (!identity) {
+            B2_TRY(idx->ids_dev.ensure((size_t)std::max<int64_t>(n_ids, 1) * sizeof(int64_t)));
+            B2_CUDA(cudaMemcpyAsync(idx->ids_dev.p, ids, (size_t)n_ids * sizeof(int64_t), cudaMemcpyHostToDevice, st));
+            ids_dev = idx->ids_dev.as<int64_t>();
+        }
+    }
+    if (idx->host) {
+        B2_TRY(host_range(idx, W, q_dev, q_dtype, nq, radius, ids_dev ? ids : nullptr, ids_dev, n_ids, st));
+    } else if (ids_dev) {
+        MatView sub;
+        B2_TRY(build_subset(idx, ids_dev, n_ids, q_dtype, sub, st));
+        B2_TRY(range_device(idx, W, sub, q_dev, q_dtype, nq, radius, st));
+    } else {
+        B2_TRY(range_device(idx, W, idx->view, q_dev, q_dtype, nq, radius, st));
+    }
+    B2_TRY(range_finish(W, ids_dev, 0, st));
+    B2_CUDA(cudaMemcpyAsync(lims, W.lims.p, (size_t)(nq + 1) * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    cudaError_t e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) { set_error("range search failed on the device: %s", cudaGetErrorString(e)); return B2_ECUDA; }
+    if (W.use_filter && W.n_dense < nq) idx->last_filter_ms = W.filter_ms;
+    const int64_t total = lims[nq];
+    *n_results = total;
+    if (total > cap) {
+        set_error("range search found %lld results, more than cap=%lld", (long long)total, (long long)cap);
+        return B2_ERANGE;
+    }
+    if (total > 0) {
+        B2_CUDA(cudaMemcpyAsync(out_d, W.out_d.p, (size_t)total * sizeof(float), cudaMemcpyDeviceToHost, st));
+        B2_CUDA(cudaMemcpyAsync(out_i, W.out_i.p, (size_t)total * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+        e = cudaStreamSynchronize(st);
+        if (e != cudaSuccess) { set_error("range search failed on the device: %s", cudaGetErrorString(e)); return B2_ECUDA; }
+    }
+    return B2_OK;
+}
+
+int b2_debug_range_stats(const b2_index* idx, int64_t* out4) {
+    if (!idx || !out4) { set_error("NULL argument"); return B2_EINVAL; }
+    const RangeWork* W = idx->range.get();
+    out4[0] = W ? W->cand_peak : 0;
+    out4[1] = W ? W->n_hits : 0;
+    out4[2] = W ? W->n_dense : 0;
+    out4[3] = W ? (int64_t)W->use_filter : 0;
     return B2_OK;
 }
 

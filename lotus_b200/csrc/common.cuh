@@ -169,6 +169,11 @@ int filter_min_splits_for_k(int k);
 int sm_count(int device);  // multiprocessor count of a device, cached
 int launch_pair_filter(const MatView& X, float thr, int part, int nparts, int32_t* pair_i, int32_t* pair_j,
                        unsigned long long* pair_count, unsigned long long cap, int device, cudaStream_t stream);
+// range search: (query, row) candidates whose filter score beats thr[query] (NaN: none), see range.cu
+int range_filter_workers(int device, int cl, int* workers);
+int range_filter_splits(int64_t nq, int64_t n, int workers, int cl);
+int launch_range_filter(const MatView& X, const void* q_filt, int64_t q_pitch, int64_t nq, int metric, const float* thr, int cluster,
+                        int workers, int2* cand, unsigned long long* count, unsigned long long cap, cudaStream_t stream);
 
 // knn_exact.cu
 int launch_prep_queries(const void* q, int q_dtype, int64_t nq, int d, void* q_filt, int filt_dtype,

@@ -181,6 +181,34 @@ struct FilterPlan {
     float q_norm_limit = INFINITY;
 };
 
+// Workspace and state of one range search (range.cu): per-query thresholds, the dense query list, the filter's candidates and
+// the verified hits, appended pass by pass (one pass over a device-resident view, one per streamed chunk).
+struct RangeWork {
+    DevBuf thr, sel, counts, cand, hit_q, hit_pos, hit_sc, keys, sc_alt, sort_tmp, lims, out_d, out_i;
+    HostBuf h_count;
+    const void* q = nullptr;  // the queries (device), as verification reads them
+    int q_dtype = B2_F32, metric = B2_METRIC_IP, filt_dtype = B2_F32;
+    int64_t nq = 0;
+    float radius = 0.f;
+    bool use_filter = false;
+    float rel_eps = 0.f, abs_eps = 0.f, q_norm_limit = INFINITY;
+    const void* q_filt = nullptr;  // the queries in the filter's type
+    int64_t q_pitch = 0;
+    int cluster = 1, workers = 0;
+    int64_t n_dense = 0;    // queries the dense path answers (sel[1 .. n_dense])
+    int64_t n_hits = 0;     // verified hits so far
+    int64_t cand_peak = 0;  // most candidates one filter launch produced
+    float filter_ms = 0.f;
+};
+// thresholds and query preparation for a search of X (for a streamed index: X.n = rows per chunk); X.filt_dtype is ignored
+int range_begin(b2_index* idx, RangeWork& W, const MatView& X, int metric, const void* q_dev, int q_dtype, int64_t nq, float radius,
+                cudaStream_t st);
+// filter + verify the rows [own_lo, X.n) of X (X.filt / filt_dtype: the filter operand; X.store: the exact rows, row pitch
+// `pitch`), reporting row j as position base + j
+int range_pass(b2_index* idx, RangeWork& W, const MatView& X, int64_t pitch, int64_t base, int64_t own_lo, cudaStream_t st);
+// sort the hits into W.lims [nq + 1], W.out_d / W.out_i [n_hits] (positions mapped through id_map, or + id_offset)
+int range_finish(RangeWork& W, const int64_t* id_map, int64_t id_offset, cudaStream_t st);
+
 }  // namespace b2
 
 struct b2_index {
@@ -215,6 +243,7 @@ struct b2_index {
     // host-resident indexes (b2_index_create_host): the rows live in pinned, mapped host memory and searches stream them
     // through a ring of device slots (host_resident.cu); `store` stays empty and `view.store` is the mapped pointer
     std::unique_ptr<b2::HostStore> host;
+    std::unique_ptr<b2::RangeWork> range;  // range search workspaces, made on the first range search
     ~b2_index();  // destroys the stream and events; the buffers free themselves
 };
 

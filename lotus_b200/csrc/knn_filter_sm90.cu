@@ -943,6 +943,119 @@ pair_i8_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
     pair_filter_body<Op::I8, CL>(tmap_q, tmap_x, p);
 }
 
+// ---- range filter (range search): same mainloop and knn schedule, the epilogue emits (query, row) candidates ----------
+// Every (query tile, corpus tile) pair is one tile of exactly one item (item_range, knn form). A lane's accumulators hold
+// two query rows; their thresholds stay in registers for the whole item. A row is a candidate when its filter score (IP:
+// <q, x>; L2: 2 <q, x> - |x|^2) is strictly above the threshold of its query; a NaN threshold (a query the exact dense path
+// answers, or a row past nq) passes nothing. Op::I8 compares the exact integer scores against the thresholds rounded down.
+struct RangeParams {
+    const float* thr;             // [nq] candidate threshold in filter-score space
+    int2* cand;                   // [cap] (query, corpus row) of each candidate, in arbitrary order
+    unsigned long long* count;    // total candidates found (may exceed cap)
+    unsigned long long cap;
+};
+constexpr int RANGE_STAGES = MAX_STAGES;
+constexpr int RANGE_SMEM = RANGE_STAGES * STAGE_BYTES + BAR_BYTES + SMEM_ALIGN_SLACK;
+
+template <Op OP, bool IS_L2, int CL>
+__device__ __forceinline__ void range_filter_body(const CUtensorMap& tmap_q, const CUtensorMap& tmap_x, const FilterParams& p,
+                                                  const RangeParams& rp) {
+    using AccT = std::conditional_t<OP == Op::I8, int32_t, float>;
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = align_smem(smem_raw);
+    const int warp = threadIdx.x >> 5;
+    const int lane = threadIdx.x & 31;
+    const Ring ring = setup_ring<RANGE_STAGES, CL>(smem, &tmap_q, &tmap_x);
+    const int n_items = num_items(p);
+    const Sched sc = make_sched<CL>();
+    if (warp < 4) {
+        setmaxnreg_dec<40>();
+        if (threadIdx.x == 0) producer_loop<OP, RANGE_STAGES, CL, 0>(&tmap_q, &tmap_x, p, ring, sc);
+    } else {
+        setmaxnreg_inc<232>();
+        const int g = (warp >> 2) - 1;
+        const int wq = warp & 3;
+        int stage = 0;
+        uint32_t phase = 0;
+        AccT acc[128];
+        uint32_t no_afrag[1][KB_AREGS];  // every K-block reads A from shared memory
+        for (int item = sc.worker; item < n_items; item += sc.n_workers) {
+            int m_tile, split, t0, t1;
+            item_range<CL>(p, sc, item, m_tile, split, t0, t1);
+            const int gi0 = m_tile * BLOCK_M + g * WG_M + wq * 16 + (lane >> 2);  // query rows gi0 and gi0 + 8 of this lane
+            AccT thr[2];
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const float tq = gi0 + 8 * h < p.nq ? __ldg(rp.thr + gi0 + 8 * h) : __int_as_float(0x7fc00000);
+                if constexpr (OP == Op::I8) thr[h] = tq != tq ? INT_MAX : __float2int_rd(tq);  // NaN: nothing passes
+                else thr[h] = tq;
+            }
+            for (int t = t0; t < t1; ++t) {
+                mma_tile<OP, RANGE_STAGES, CL, 0>(acc, no_afrag, false, ring, p.num_kb, g, sc.cta, stage, phase);
+                const int col0 = t * BLOCK_N + 2 * (lane & 3);
+#pragma unroll
+                for (int c = 0; c < BLOCK_N / 16; ++c) {  // 16-column chunks: acc[8c .. 8c + 7]
+                    uint32_t mask = 0;
+#pragma unroll
+                    for (int h = 0; h < 8; ++h) {
+                        const int i = 8 * c + h;
+                        const int gj = col0 + 8 * (i >> 2) + (i & 1);
+                        const bool valid = gj < p.n;
+                        bool pass;
+                        if constexpr (OP == Op::I8) {
+                            pass = valid && i8_score<IS_L2>(acc[i], p, gj, valid) > thr[(i >> 1) & 1];
+                        } else {
+                            float s = acc[i];
+                            if constexpr (IS_L2) {
+                                if (valid) s = fmaf(2.f, s, -__ldg(p.xnorm + gj));
+                            }
+                            pass = valid && s > thr[(i >> 1) & 1];
+                        }
+                        mask |= pass ? 1u << h : 0u;
+                    }
+                    if (!__any_sync(0xffffffffu, mask != 0)) continue;
+                    // warp-aggregated append: one atomic per warp and chunk, each lane writes its candidates contiguously
+                    const int cnt = __popc(mask);
+                    int incl = cnt;
+#pragma unroll
+                    for (int off = 1; off < 32; off <<= 1) {
+                        const int v = __shfl_up_sync(0xffffffffu, incl, off);
+                        if (lane >= off) incl += v;
+                    }
+                    const int total = __shfl_sync(0xffffffffu, incl, 31);
+                    unsigned long long base = 0;
+                    if (lane == 31) base = atomicAdd(rp.count, (unsigned long long)total);
+                    base = __shfl_sync(0xffffffffu, base, 31) + (unsigned long long)(incl - cnt);
+#pragma unroll
+                    for (int h = 0; h < 8; ++h) {
+                        if (mask & (1u << h)) {
+                            const int i = 8 * c + h;
+                            if (base < rp.cap) rp.cand[base] = make_int2(gi0 + 8 * ((i >> 1) & 1), col0 + 8 * (i >> 2) + (i & 1));
+                            ++base;
+                        }
+                    }
+                }
+            }
+        }
+    }
+    teardown_ring<CL>();
+}
+
+template <Op OP, bool IS_L2, int CL>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+range_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_x, const FilterParams p,
+                    const RangeParams rp) {
+    range_filter_body<OP, IS_L2, CL>(tmap_q, tmap_x, p, rp);
+}
+
+// the int8 range filter (IGMMA), an entry of its own like knn_i8_filter_kernel
+template <bool IS_L2, int CL>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+range_i8_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_x, const FilterParams p,
+                       const RangeParams rp) {
+    range_filter_body<Op::I8, IS_L2, CL>(tmap_q, tmap_x, p, rp);
+}
+
 // ---- host side ---------------------------------------------------------------------------------------------
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                     const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
@@ -1378,6 +1491,133 @@ int launch_pair_filter(const MatView& X, float thr, int part, int nparts, int32_
         default:  // Op::F16
             return two_cta ? launch_cluster(pair_filter_kernel<Op::F16, 2>, grid, PAIR_SMEM, 2, tq, tx, p, stream)
                            : launch_cluster(pair_filter_kernel<Op::F16, 1>, grid, PAIR_SMEM, 1, tq, tx, p, stream);
+    }
+}
+
+namespace {
+
+template <typename Kern>
+int launch_range_cluster(Kern kern, int grid, int cl, const CUtensorMap& tq, const CUtensorMap& tx, const FilterParams& p,
+                         const RangeParams& rp, cudaStream_t stream) {
+    B2_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, RANGE_SMEM));
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3((unsigned)grid);
+    cfg.blockDim = dim3(NUM_THREADS);
+    cfg.dynamicSmemBytes = RANGE_SMEM;
+    cfg.stream = stream;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = (unsigned)cl;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    B2_CUDA(cudaLaunchKernelEx(&cfg, kern, tq, tx, p, rp));
+    B2_LAUNCH_CHECK();
+    g_stats[ST_FILTER_LAUNCHES]++;
+    return B2_OK;
+}
+
+template <bool IS_L2, int CL>
+int launch_range_op(Op op, int grid, const CUtensorMap& tq, const CUtensorMap& tx, const FilterParams& p, const RangeParams& rp,
+                    cudaStream_t stream) {
+    switch (op) {
+        case Op::TF32: return launch_range_cluster(range_filter_kernel<Op::TF32, IS_L2, CL>, grid, CL, tq, tx, p, rp, stream);
+        case Op::BF16: return launch_range_cluster(range_filter_kernel<Op::BF16, IS_L2, CL>, grid, CL, tq, tx, p, rp, stream);
+        case Op::I8: return launch_range_cluster(range_i8_filter_kernel<IS_L2, CL>, grid, CL, tq, tx, p, rp, stream);
+        default: return launch_range_cluster(range_filter_kernel<Op::F16, IS_L2, CL>, grid, CL, tq, tx, p, rp, stream);  // Op::F16
+    }
+}
+
+template <int CL>
+int launch_range_cl(bool is_l2, Op op, int grid, const CUtensorMap& tq, const CUtensorMap& tx, const FilterParams& p,
+                    const RangeParams& rp, cudaStream_t stream) {
+    return is_l2 ? launch_range_op<true, CL>(op, grid, tq, tx, p, rp, stream) : launch_range_op<false, CL>(op, grid, tq, tx, p, rp, stream);
+}
+
+}  // namespace
+
+// Workers of one persistent range-filter launch in clusters of `cl` on the current device, which is `device` (CTA pairs in
+// cluster mode, two per cluster of four), cached per device.
+int range_filter_workers(int device, int cl, int* workers) {
+    static int cached[64][3] = {};
+    const int ci = cl == 1 ? 0 : cl == 2 ? 1 : 2;
+    int* slot = (device >= 0 && device < 64) ? &cached[device][ci] : nullptr;
+    if (slot && *slot) {
+        *workers = *slot;
+        return B2_OK;
+    }
+    switch (cl) {
+        case 1: B2_TRY(co_resident_clusters(range_filter_kernel<Op::BF16, false, 1>, RANGE_SMEM, 1, workers)); break;
+        case 2: B2_TRY(co_resident_clusters(range_filter_kernel<Op::BF16, false, 2>, RANGE_SMEM, 2, workers)); break;
+        default: B2_TRY(co_resident_clusters(range_filter_kernel<Op::BF16, false, FILTER_CL>, RANGE_SMEM, FILTER_CL, workers)); break;
+    }
+    if (cl > 2) *workers *= cl / 2;
+    if (slot) *slot = *workers;
+    return B2_OK;
+}
+
+// Corpus splits of a range filter: items carry no list, so a split costs no warm-up; the corpus is cut only as far as it
+// takes to give every worker an item (and not so far that a split has no tile).
+int range_filter_splits(int64_t nq, int64_t n, int workers, int cl) {
+    const int64_t n_mtiles = ceil_div(nq, BLOCK_M);
+    int64_t units = cl > 1 ? ceil_div(n_mtiles, 2) : n_mtiles;
+    if (cl > 2) units += units & 1;
+    const int64_t n_ntiles = ceil_div(n, BLOCK_N);
+    int64_t s = std::max<int64_t>(1, std::min<int64_t>(n_ntiles, ceil_div(workers, units)));
+    s = ceil_div(n_ntiles, ceil_div(n_ntiles, s));  // every split receives tiles
+    return (int)s;
+}
+
+// Candidates (query, row) of a range search: rows of X whose filter score beats thr[query] (filter-score space, see
+// RangeParams). cand (device, capacity cap) receives them in arbitrary order and *count (device, zeroed by the caller) the
+// total found, which may exceed cap. cluster / workers as filter_cluster / range_filter_workers chose them.
+int launch_range_filter(const MatView& X, const void* q_filt, int64_t q_pitch, int64_t nq, int metric, const float* thr, int cluster,
+                        int workers, int2* cand, unsigned long long* count, unsigned long long cap, cudaStream_t stream) {
+    if (nq <= 0 || X.n <= 0) return B2_OK;
+    if (X.n > 0x7fffff00LL || nq > 0x7fffff00LL) {
+        set_error("matrix too large for 32-bit row ids (n=%lld nq=%lld)", (long long)X.n, (long long)nq);
+        return B2_ERANGE;
+    }
+    const Op op = filter_op(X.filt_dtype);
+    const int kb_elems = KB_BYTES / op_bytes(op);
+    const bool is_l2 = metric == B2_METRIC_L2;
+    if (is_l2 && (!X.norm2 || (op == Op::I8 && !X.norm2_i8))) {
+        set_error("internal: L2 range filter without row norms");
+        return B2_EINVAL;
+    }
+    if ((cluster != 1 && cluster != 2 && cluster != FILTER_CL) || workers <= 0 || (cluster > 2 && workers % 2 != 0)) {
+        set_error("internal: bad range filter launch (%d workers of %d CTAs)", workers, cluster);
+        return B2_EINVAL;
+    }
+    CUtensorMap tq, tx;
+    B2_TRY(make_tmap(&tq, q_filt, op, nq, X.d, q_pitch, BLOCK_M));
+    B2_TRY(make_tmap(&tx, X.filt, op, X.n, X.d, X.filt_pitch, BLOCK_N / cluster));
+    FilterParams p;
+    memset(&p, 0, sizeof(p));
+    p.xnorm = X.norm2;
+    p.xnorm_i = X.norm2_i8;
+    p.nq = (int32_t)nq;
+    p.n = (int32_t)X.n;
+    p.num_kb = (int32_t)ceil_div(X.d, kb_elems);
+    p.n_mtiles = (int32_t)ceil_div(nq, BLOCK_M);
+    p.n_munits = cluster > 1 ? (p.n_mtiles + 1) / 2 : p.n_mtiles;
+    p.n_munits += cluster > 2 ? (p.n_munits & 1) : 0;  // clusters of four: an even number of units (a surplus one writes nothing)
+    p.n_ntiles = (int32_t)ceil_div(X.n, BLOCK_N);
+    p.n_splits = range_filter_splits(nq, X.n, workers, cluster);
+    p.tiles_per_split = (int32_t)ceil_div(p.n_ntiles, p.n_splits);
+    p.units_whole = 0;
+    RangeParams rp;
+    rp.thr = thr;
+    rp.cand = cand;
+    rp.count = count;
+    rp.cap = cap;
+    const int64_t items = (int64_t)p.n_munits * p.n_splits;
+    const int grid = (cluster > 1 ? 2 : 1) * (int)std::min<int64_t>(items, workers);
+    switch (cluster) {
+        case 1: return launch_range_cl<1>(is_l2, op, grid, tq, tx, p, rp, stream);
+        case 2: return launch_range_cl<2>(is_l2, op, grid, tq, tx, p, rp, stream);
+        default: return launch_range_cl<FILTER_CL>(is_l2, op, grid, tq, tx, p, rp, stream);
     }
 }
 

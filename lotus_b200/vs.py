@@ -210,6 +210,30 @@ class MultiDeviceIndex:
         parts = list(self.pool.map(one, range(len(self.shards))))
         return merge_shard_lists([p[0] for p in parts], [p[1] for p in parts], self.metric)
 
+    def range_search(self, q: np.ndarray, radius: float, q_dtype: int = nv.F32, ids: np.ndarray | None = None):
+        """(lims, D, I) as `_native.Index.range_search`. Each shard answers for its rows (an ids subset: the distinct ids it
+        holds); the hits are then ordered per query by row id, or with ids by position in `ids`, where a repeated id
+        contributes one hit per occurrence."""
+        nq = len(q)
+        ids_a = None if ids is None else np.asarray(ids, dtype=np.int64)
+        if ids_a is not None and len(ids_a) and (ids_a.min() < 0 or ids_a.max() >= self.n):
+            raise nv.NativeError(nv.ERANGE, f"ids contains a position outside [0, {self.n})")
+        uniq = None if ids_a is None else np.unique(ids_a)
+
+        def one(g):
+            lo, hi = self.bounds[g]
+            if uniq is None:
+                lims, D, I = self.shards[g].range_search(q, radius, q_dtype)
+            else:
+                mine = uniq[(uniq >= lo) & (uniq < hi)] - lo
+                if len(mine) == 0:
+                    return np.empty(0, np.int64), np.empty(0, np.float32), np.empty(0, np.int64)
+                lims, D, I = self.shards[g].range_search(q, radius, q_dtype, ids=mine)
+            return np.repeat(np.arange(nq, dtype=np.int64), np.diff(lims)), D, I + lo
+
+        parts = list(self.pool.map(one, range(len(self.shards))))
+        return combine_range_hits(nq, [p[0] for p in parts], [p[1] for p in parts], [p[2] for p in parts], ids_a)
+
     def gather(self, ids) -> np.ndarray:
         ids = np.asarray(ids, dtype=np.int64)
         if len(ids) and (ids.min() < 0 or ids.max() >= self.n):
@@ -251,6 +275,29 @@ def merge_shard_lists(D_parts: list, I_parts: list, metric: int):
     key = np.where(I >= 0, D if metric == nv.METRIC_L2 else -D, np.inf)
     sel = np.argsort(key, axis=1, kind="stable")[:, :k]
     return np.take_along_axis(D, sel, axis=1), np.take_along_axis(I, sel, axis=1)
+
+
+def combine_range_hits(nq: int, q_parts: list, d_parts: list, row_parts: list, ids: "np.ndarray | None" = None):
+    """Per-shard range hits (query, score, global row) -> (lims[nq+1], D, I) ordered per query by row id; with `ids`, each
+    hit row is expanded to every position of `ids` holding it, ordered per query by position and reported as ids[position]."""
+    qs = np.concatenate(q_parts).astype(np.int64, copy=False) if q_parts else np.empty(0, np.int64)
+    D = np.concatenate(d_parts).astype(np.float32, copy=False) if d_parts else np.empty(0, np.float32)
+    rows = np.concatenate(row_parts).astype(np.int64, copy=False) if row_parts else np.empty(0, np.int64)
+    if ids is None:
+        key, I = rows, rows
+    else:
+        order = np.argsort(ids, kind="stable")
+        sid = ids[order]
+        left = np.searchsorted(sid, rows, "left")
+        cnt = np.searchsorted(sid, rows, "right") - left
+        rep = np.repeat(np.arange(len(rows)), cnt)
+        within = np.arange(len(rep)) - np.repeat(np.cumsum(cnt) - cnt, cnt)
+        key = order[left[rep] + within]  # positions in ids
+        qs, D, I = qs[rep], D[rep], ids[key]
+    o = np.lexsort((key, qs))
+    lims = np.zeros(nq + 1, dtype=np.int64)
+    np.cumsum(np.bincount(qs, minlength=nq), out=lims[1:])
+    return lims, D[o], I[o]
 
 
 def _free_device_bytes(device: int) -> int:
@@ -493,6 +540,26 @@ class B200VS(VS):
                 raise ValueError(e.msg) from e
             raise
         return RMOutput(distances=out_s.cpu().numpy(), indices=out_i.cpu().numpy())
+
+    def range_search(self, query_vectors: Any, radius: float, ids: Any = None):
+        """faiss IndexFlat.range_search(x, radius) over the loaded index: (lims[Q+1] int64, D float32, I int64), query i's
+        hits at [lims[i], lims[i+1]) in ascending id. IP keeps rows whose score is strictly greater than `radius`; L2 those
+        whose squared distance is strictly less. D holds the values __call__ reports. ids: only those rows, as a temporary
+        index over vecs[ids] (faiss_vs.py:57-72): hits follow the order of `ids`, a repeated id once per occurrence. Queries
+        as __call__ accepts them."""
+        if self.b2_index is None or self.index_dir is None:
+            raise ValueError("Index not loaded")
+        ids_a = None if ids is None else np.asarray(list(ids) if not isinstance(ids, np.ndarray) else ids, dtype=np.int64)
+        q, code, _ = _to_host_matrix(query_vectors, False, exact_bf16_ok=self.b2_index.dtype == nv.BF16, scratch=self._scratch,
+                                     pass_f16=True, pass_i8=True)
+        if q.shape[1] != self.b2_index.d:
+            raise ValueError(f"query dimension {q.shape[1]} does not match the index dimension {self.b2_index.d}")
+        try:
+            return self.b2_index.range_search(q, float(radius), code, ids=ids_a)
+        except nv.NativeError as e:
+            if e.code in (nv.EINVAL, nv.ERANGE):
+                raise ValueError(e.msg) from e
+            raise
 
     # -- extensions used by the re-registered operators --------------------------------------------------------------
     def _refuse_host(self, what: str) -> None:
