@@ -137,6 +137,20 @@ B2_API int b2_index_search_dev(b2_index* idx, const void* q_dev, int64_t nq, int
                         const int64_t* ids_dev, int64_t n_ids, int64_t id_offset, float* out_scores_dev,
                         int64_t* out_idx_dev, void* stream);
 
+/* Masked search: only the rows a bitmap selects take part, searched in place. mask holds ceil(n / 32) little-endian 32-bit
+ * words, bit (j & 31) of word (j >> 5) set = row j takes part; bits at or past n are ignored. The result is that of
+ * b2_index_search with ids = the ascending list of the set rows, bit for bit (indices and score bits, and the -1 / -+FLT_MAX
+ * padding when fewer than k rows are selected, an all-zero mask included), but no copy of the subset is made: the filter
+ * kernel sweeps the whole index and leaves the cleared rows out, so a subset of a device-resident index costs no device
+ * memory beyond the bitmap and one of a host-resident index no gather on the host. It sweeps all n rows whatever the mask
+ * selects. Every dtype, both metrics, both residencies, k up to b2_max_k(). HOST buffers. */
+B2_API int b2_index_search_masked(b2_index* idx, const void* q, int64_t nq, int32_t q_dtype, int32_t k, const uint32_t* mask,
+                                  float* out_scores, int64_t* out_idx);
+/* DEVICE buffers (mask_dev included); id_offset is added to every reported id, as in b2_index_search_dev. */
+B2_API int b2_index_search_masked_dev(b2_index* idx, const void* q_dev, int64_t nq, int32_t q_dtype, int32_t k,
+                                      const uint32_t* mask_dev, int64_t id_offset, float* out_scores_dev, int64_t* out_idx_dev,
+                                      void* stream);
+
 /* k-way merge of g per-shard result lists: scores[g,nq,k], idx[g,nq,k] (each list sorted best first, shard
  * s holding ids below those of shard s+1) -> out[nq,k]. DEVICE buffers on `device`. */
 B2_API int b2_merge_topk_dev(const float* scores_dev, const int64_t* idx_dev, int32_t g, int64_t nq, int32_t k,
@@ -245,6 +259,11 @@ B2_API int b2_debug_filter_plan(int64_t nq, int64_t n, int32_t k, int32_t num_sm
  * chunk. For testing; not part of the search path. */
 B2_API int b2_debug_filter_lists(b2_index* idx, const void* q, int64_t nq, int32_t q_dtype, int32_t k, int32_t top1, int32_t level,
                           int32_t* plan, float* rel_eps, float* cand_score, int32_t* cand_id, float* cand_thr);
+/* b2_debug_filter_lists for a masked search (mask: HOST, as b2_index_search_masked takes it): no cleared row is on any list,
+ * and a list's bound holds for the selected rows it discarded. */
+B2_API int b2_debug_filter_lists_masked(b2_index* idx, const void* q, int64_t nq, int32_t q_dtype, int32_t k, int32_t level,
+                                        const uint32_t* mask, int32_t* plan, float* rel_eps, float* cand_score, int32_t* cand_id,
+                                        float* cand_thr);
 /* The chunking of a host-resident index of n rows (no device work): *chunk_rows rows per chunk (a multiple of 256 unless
  * one chunk holds every row), *n_chunks chunks, *slots device slots of the ring. Chunk c owns the rows
  * [c * chunk_rows, min(n, (c + 1) * chunk_rows)); it streams chunk_rows rows from min(c * chunk_rows, n - chunk_rows) on,

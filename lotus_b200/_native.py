@@ -25,6 +25,7 @@ SYMBOLS = [
     "b2_connected_components", "b2_kmeans", "b2_kmeans_assign", "b2_kmeans_accumulate", "b2_kmeans_assign_dev", "b2_kmeans_accumulate_dev", "b2_stats", "b2_stats_reset", "b2_last_filter_ms", "b2_host_f32_to_bf16", "b2_host_bf16_to_f32", "b2_debug_filter_plan",
     "b2_debug_filter_lists", "b2_debug_filter_eps", "b2_index_create_host", "b2_index_resident", "b2_debug_stream_plan",
     "b2_debug_stream_times", "b2_index_range_search", "b2_debug_range_stats",
+    "b2_index_search_masked", "b2_index_search_masked_dev", "b2_debug_filter_lists_masked",
 ]
 
 
@@ -74,6 +75,12 @@ def lib() -> ctypes.CDLL:
     L.b2_index_search.argtypes = [vp, vp, i64, i32, i32, vp, i64, vp, vp]
     L.b2_index_search_dev.restype = c.c_int
     L.b2_index_search_dev.argtypes = [vp, vp, i64, i32, i32, vp, i64, i64, vp, vp, vp]
+    L.b2_index_search_masked.restype = c.c_int
+    L.b2_index_search_masked.argtypes = [vp, vp, i64, i32, i32, vp, vp, vp]
+    L.b2_index_search_masked_dev.restype = c.c_int
+    L.b2_index_search_masked_dev.argtypes = [vp, vp, i64, i32, i32, vp, i64, vp, vp, vp]
+    L.b2_debug_filter_lists_masked.restype = c.c_int
+    L.b2_debug_filter_lists_masked.argtypes = [vp, vp, i64, i32, i32, i32, vp, c.POINTER(i32), c.POINTER(f32), vp, vp, vp]
     L.b2_merge_topk_dev.restype = c.c_int
     L.b2_merge_topk_dev.argtypes = [vp, vp, i32, i64, i32, i32, i32, vp, vp, vp]
     L.b2_index_search_packed_dev.restype = c.c_int
@@ -229,6 +236,56 @@ def stored_to_f32(a: np.ndarray, code: int) -> np.ndarray:
     raise ValueError(f"unknown element type code {code}")
 
 
+# ---- row bitmaps of a masked search (host logic only) -------------------------------------------------------------------
+def mask_nwords(n: int) -> int:
+    return (int(n) + 31) // 32
+
+
+def pack_mask(mask, n: int) -> np.ndarray:
+    """The bitmap of a masked search over n rows as the C-ABI takes it: ceil(n / 32) uint32 words, bit j & 31 of word j >> 5
+    set = row j takes part. `mask` is a bool array of length n, or such words already (returned as they are)."""
+    a = np.asarray(mask)
+    if a.dtype == np.uint32:
+        if a.ndim != 1 or len(a) != mask_nwords(n):
+            raise ValueError(f"a packed mask over {n} rows has {mask_nwords(n)} uint32 words, got shape {a.shape}")
+        return np.ascontiguousarray(a)
+    if a.dtype != np.bool_ or a.ndim != 1 or len(a) != n:
+        raise ValueError(f"mask must be a bool array of length {n} or packed uint32 words, got {a.dtype} of shape {a.shape}")
+    by = np.zeros(4 * mask_nwords(n), dtype=np.uint8)
+    packed = np.packbits(a, bitorder="little")
+    by[:len(packed)] = packed
+    return by.view("<u4").astype(np.uint32, copy=False)
+
+
+def unpack_mask(words: np.ndarray, n: int) -> np.ndarray:
+    """bool[n] of packed mask words (the inverse of pack_mask)."""
+    by = np.ascontiguousarray(words, dtype="<u4").view(np.uint8)
+    return np.unpackbits(by, bitorder="little")[:n].astype(np.bool_)
+
+
+def strictly_ascending(ids: np.ndarray) -> bool:
+    """Whether ids has no repeats and is in ascending order: the order of such a subset is the row order, so a masked search
+    over its bitmap has the tie semantics of the temporary index over x[ids]."""
+    ids = np.asarray(ids)
+    return len(ids) < 2 or bool((ids[1:] > ids[:-1]).all())
+
+
+def ids_to_mask(ids: np.ndarray, n: int) -> np.ndarray:
+    """Packed bitmap over n rows with the bits of `ids` set; ids outside [0, n) raise NativeError(ERANGE) like a search."""
+    ids = np.asarray(ids, dtype=np.int64)
+    if len(ids) and (ids.min() < 0 or ids.max() >= n):
+        raise NativeError(ERANGE, f"ids contains a position outside [0, {n})")
+    b = np.zeros(n, dtype=np.bool_)
+    b[ids] = True
+    return pack_mask(b, n)
+
+
+def slice_mask(words: np.ndarray, n: int, lo: int, hi: int) -> np.ndarray:
+    """The packed bitmap of the rows [lo, hi) of a bitmap over n rows, re-based so that row lo is bit 0 (shard bounds need not
+    fall on word boundaries)."""
+    return pack_mask(unpack_mask(words, n)[lo:hi], hi - lo)
+
+
 def _ptr(a: Optional[np.ndarray]):
     return None if a is None else ctypes.c_void_p(a.ctypes.data)
 
@@ -264,6 +321,7 @@ class Index:
             else:
                 check(L.b2_index_create(_ptr(x) if n else None, n, d, dtype, metric, device, 0, ctypes.byref(self._h)))
         self.n, self.d, self.dtype, self.metric, self.device = int(n), int(d), dtype, metric, device
+        self.ring_bytes = (int(ring_bytes) or (1 << 30)) if residency == "host" else 0  # 0 = the library default, 1 GiB
 
     def close(self) -> None:
         if getattr(self, "_h", None) is not None and self._h.value:
@@ -307,6 +365,26 @@ class Index:
         check(lib().b2_index_search(self._h, _ptr(q) if nq else None, nq, q_dtype, k, _ptr(ids_a),
                                     0 if ids_a is None else len(ids_a), _ptr(D), _ptr(I)))
         return D, I
+
+    def search_masked(self, q: np.ndarray, k: int, q_dtype: int, mask):
+        """search(q, k, q_dtype, ids=np.flatnonzero(mask)), bit for bit, without a gathered copy of the subset: the filter sweeps
+        the whole index and leaves the cleared rows out. mask: bool[n], or packed uint32 words (pack_mask)."""
+        q = np.ascontiguousarray(q)
+        nq = q.shape[0]
+        if nq and q.shape[1] != self.d:
+            raise ValueError(f"query dimension {q.shape[1]} != index dimension {self.d}")
+        words = pack_mask(mask, self.n)
+        D = np.empty((nq, k), dtype=np.float32)
+        I = np.empty((nq, k), dtype=np.int64)
+        check(lib().b2_index_search_masked(self._h, _ptr(q) if nq else None, nq, q_dtype, k, _ptr(words) if self.n else None,
+                                           _ptr(D), _ptr(I)))
+        return D, I
+
+    def search_masked_dev(self, q_ptr: int, nq: int, k: int, q_dtype: int, mask_ptr: int, out_scores_ptr: int, out_idx_ptr: int,
+                          id_offset: int = 0, stream: int = 0) -> None:
+        check(lib().b2_index_search_masked_dev(self._h, ctypes.c_void_p(q_ptr), nq, q_dtype, k, ctypes.c_void_p(mask_ptr), id_offset,
+                                               ctypes.c_void_p(out_scores_ptr), ctypes.c_void_p(out_idx_ptr),
+                                               ctypes.c_void_p(stream) if stream else None))
 
     def range_search(self, q: np.ndarray, radius: float, q_dtype: int = F32, ids: Optional[np.ndarray] = None,
                      cap: Optional[int] = None):
@@ -369,10 +447,11 @@ class Index:
         return out
 
     def filter_lists(self, q: np.ndarray, k: int, q_dtype: int = F32, top1: bool = False, level: int = 0,
-                     plan_only: bool = False) -> dict:
+                     plan_only: bool = False, mask=None) -> dict:
         """The filter kernel's raw candidate lists for host queries, run as a search (or, with top1, the k-means assignment)
         runs it: the plan (use_filter, kp, n_splits, units_whole, two_cta, cluster, two_level, filt_dtype, rel_eps) plus, unless
-        plan_only or the plan declines the filter, score/id [nq, n_splits, 2, kp/2] and thr [nq, n_splits, 2]."""
+        plan_only or the plan declines the filter, score/id [nq, n_splits, 2, kp/2] and thr [nq, n_splits, 2]. mask: the
+        lists of a masked search (search_masked) instead."""
         q = np.ascontiguousarray(q)
         nq = q.shape[0]
         if q.ndim != 2 or q.shape[1] != self.d:
@@ -380,7 +459,17 @@ class Index:
         plan = (ctypes.c_int32 * 8)()
         eps = ctypes.c_float()
         L = lib()
-        check(L.b2_debug_filter_lists(self._h, _ptr(q), nq, q_dtype, k, int(top1), level, plan, ctypes.byref(eps), None, None, None))
+        if mask is not None:
+            if top1:
+                raise ValueError("the k-means assignment takes no mask")
+            words = pack_mask(mask, self.n)
+
+            def run(*bufs):
+                return L.b2_debug_filter_lists_masked(self._h, _ptr(q), nq, q_dtype, k, level, _ptr(words), plan, ctypes.byref(eps), *bufs)
+        else:
+            def run(*bufs):
+                return L.b2_debug_filter_lists(self._h, _ptr(q), nq, q_dtype, k, int(top1), level, plan, ctypes.byref(eps), *bufs)
+        check(run(None, None, None))
         out = {"use_filter": bool(plan[0]), "kp": plan[1], "n_splits": plan[2], "units_whole": plan[3], "two_cta": plan[4] > 1,
                "cluster": plan[4],
                "two_level": bool(plan[5]), "filt_dtype": plan[6], "rel_eps": float(eps.value)}
@@ -390,8 +479,7 @@ class Index:
         sc = np.empty((nq, ns, 2, kph), dtype=np.float32)
         ids = np.empty((nq, ns, 2, kph), dtype=np.int32)
         thr = np.empty((nq, ns, 2), dtype=np.float32)
-        check(L.b2_debug_filter_lists(self._h, _ptr(q), nq, q_dtype, k, int(top1), level, plan, ctypes.byref(eps), _ptr(sc),
-                                      _ptr(ids), _ptr(thr)))
+        check(run(_ptr(sc), _ptr(ids), _ptr(thr)))
         out.update(score=sc, id=ids, thr=thr)
         return out
 

@@ -146,6 +146,17 @@ __global__ void fill_pad_kernel(float* sc, int64_t* id, int64_t total, float pad
     }
 }
 
+// out[w] = the 32 mask bits from bit0 + 32 w on, for w < words (bits at or past nbits read as zero): the mask of a streamed
+// corpus chunk that does not start on a word boundary
+__global__ void mask_slice_kernel(const uint32_t* mask, int64_t bit0, int64_t nbits, int64_t words, uint32_t* out) {
+    const int64_t src_words = (nbits + 31) >> 5;
+    for (int64_t w = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; w < words; w += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t b = bit0 + 32 * w, i = b >> 5;
+        const uint32_t lo = i < src_words ? mask[i] : 0u, hi = i + 1 < src_words ? mask[i + 1] : 0u;
+        out[w] = __funnelshift_r(lo, hi, (uint32_t)(b & 31));
+    }
+}
+
 // The filter run of a search: for an fp32 store with a bf16 copy (X.filt16) and a small k it is the FIRST level of a two-level
 // search (bf16 filter, longer candidate list). Every caller filters exactly as planned here; b2_debug_filter_plan reports it.
 int plan_filter(const MatView& X_in, const void* q, int q_dtype, int64_t nq, int k, bool top1, int device, FilterPlan& p,
@@ -571,6 +582,19 @@ static int stream_filter_fold(b2_index* idx, HostRows& H, const FilterPlan& p, c
         pc.X.store = pc.X.filt;
         pc.X.norm2 = p.X.norm2 + base;
         pc.X.norm2_i8 = p.X.norm2_i8 ? p.X.norm2_i8 + base : nullptr;
+        if (p.X.mask) {
+            // the chunk's rows start at a word of the mask, except those of a last chunk that re-streams its predecessor's tail
+            if (base % 32 == 0) {
+                pc.X.mask = p.X.mask + base / 32;
+            } else {
+                const int64_t words = ceil_div(R, 32);
+                B2_TRY(hs.mask_slice.ensure((size_t)words * sizeof(uint32_t)));
+                mask_slice_kernel<<<(unsigned)std::min<int64_t>(ceil_div(words, 256), 1024), 256, 0, st>>>(p.X.mask, base, H.n, words,
+                                                                                                      hs.mask_slice.as<uint32_t>());
+                B2_LAUNCH_CHECK();
+                pc.X.mask = hs.mask_slice.as<uint32_t>();
+            }
+        }
         B2_CUDA(cudaEventRecord(hs.ev[4 * ch + 2], st));
         B2_TRY(run_filter(idx, pc, c, metric, st));
         B2_CUDA(cudaEventRecord(hs.ev[4 * ch + 3], st));
@@ -599,8 +623,10 @@ static void stream_times_add(b2_index* idx, int nc) {
 
 // The streamed search of the rows H (level as in search_core: level 1 is the tf32 second level of an fp32 store, which streams
 // the fp32 rows). Results are those of search_core over the same rows in device memory, bit for bit.
+// mask: MatView::mask over the rows of H (null = every row).
 static int stream_search(b2_index* idx, HostRows& H, int metric, const void* q_dev, int q_dtype, int64_t nq, int k,
-                         const int64_t* id_map, int64_t id_offset, float* out_sc, int64_t* out_id, cudaStream_t st, int level) {
+                         const int64_t* id_map, int64_t id_offset, float* out_sc, int64_t* out_id, cudaStream_t st, int level,
+                         const uint32_t* mask = nullptr) {
     HostStore& hs = *idx->host;
     if (level == 0) {
         idx->last_filter_ms = -1.f;
@@ -613,9 +639,11 @@ static int stream_search(b2_index* idx, HostRows& H, int metric, const void* q_d
         B2_LAUNCH_CHECK();
         return B2_OK;
     }
-    const MatView Xw = host_view(H);
+    MatView Xw = host_view(H);
+    Xw.mask = mask;
     FilterPlan p;
     B2_TRY(host_plan(idx, H, q_dev, q_dtype, nq, k, level, p));
+    p.X.mask = mask;
     const int cap = p.use_filter ? finalize_capacity(p.kp, k) : 0;
     if (!p.use_filter || cap == 0) {
         // the dense path over every row, read through the mapped pointer
@@ -685,7 +713,7 @@ static int stream_search(b2_index* idx, HostRows& H, int metric, const void* q_d
         int* err = reinterpret_cast<int*>(idx->scalar.as<char>() + 16);
         B2_TRY(launch_gather_rows(q_dev, q_dtype, H.d, idx->defer.as<int64_t>(), n_deferred, nq, idx->q_sub.p, err, st));
         B2_TRY(stream_search(idx, H, metric, idx->q_sub.p, q_dtype, n_deferred, k, id_map, id_offset, idx->sub_sc.as<float>(),
-                             idx->sub_id.as<int64_t>(), st, /*level=*/1));
+                             idx->sub_id.as<int64_t>(), st, /*level=*/1, mask));
         scatter_rows_kernel<<<(unsigned)ceil_div(n_deferred * k, 256), 256, 0, st>>>(idx->defer.as<int64_t>(), n_deferred, k,
                                                                                     idx->sub_sc.as<float>(), idx->sub_id.as<int64_t>(),
                                                                                     out_sc, out_id);
@@ -1109,6 +1137,68 @@ int b2_index_search(b2_index* idx, const void* q, int64_t nq, int32_t q_dtype, i
     return B2_OK;
 }
 
+// ---- masked search: the rows a bitmap selects, searched in place (no gathered copy of the subset) ----------------------------
+static int check_masked_args(b2_index* idx, const void* q, int64_t nq, int32_t q_dtype, int32_t k, const uint32_t* mask) {
+    if (!idx && b2_device_count() == 0) { set_error("no CUDA device: libb2lotus has no CPU fallback"); return B2_ENODEV; }
+    B2_TRY(check_search_args(idx, q, nq, q_dtype, k));
+    if (!mask && idx->n > 0) { set_error("mask is NULL"); return B2_EINVAL; }
+    return B2_OK;
+}
+
+// mask_dev: ceil(n / 32) words on the index's device
+static int masked_search(b2_index* idx, const void* q_dev, int q_dtype, int64_t nq, int k, const uint32_t* mask_dev, int64_t id_offset,
+                         float* out_sc, int64_t* out_id, cudaStream_t st) {
+    if (idx->host)
+        return stream_search(idx, idx->host->main, idx->metric, q_dev, q_dtype, nq, k, nullptr, id_offset, out_sc, out_id, st, 0, mask_dev);
+    MatView X = idx->view;
+    X.mask = mask_dev;
+    return search_core(idx, X, idx->metric, q_dev, q_dtype, nq, k, nullptr, id_offset, out_sc, out_id, st);
+}
+
+static int upload_mask(b2_index* idx, const uint32_t* mask, cudaStream_t st) {
+    const size_t bytes = (size_t)ceil_div(idx->n, 32) * sizeof(uint32_t);
+    B2_TRY(idx->mask_dev.ensure(std::max<size_t>(bytes, 4)));
+    if (bytes) B2_CUDA(cudaMemcpyAsync(idx->mask_dev.p, mask, bytes, cudaMemcpyHostToDevice, st));
+    return B2_OK;
+}
+
+int b2_index_search_masked_dev(b2_index* idx, const void* q_dev, int64_t nq, int32_t q_dtype, int32_t k, const uint32_t* mask_dev,
+                               int64_t id_offset, float* out_scores_dev, int64_t* out_idx_dev, void* stream) {
+    B2_TRY(check_masked_args(idx, q_dev, nq, q_dtype, k, mask_dev));
+    if (nq == 0) return B2_OK;
+    if (!out_scores_dev || !out_idx_dev) { set_error("output buffers are NULL"); return B2_EINVAL; }
+    DeviceGuard guard(idx->device);
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    B2_TRY(adapt_queries(idx, q_dev, q_dtype, nq, st));
+    B2_TRY(masked_search(idx, q_dev, q_dtype, nq, k, mask_dev, id_offset, out_scores_dev, out_idx_dev, st));
+    B2_CUDA(cudaStreamSynchronize(st));
+    return B2_OK;
+}
+
+int b2_index_search_masked(b2_index* idx, const void* q, int64_t nq, int32_t q_dtype, int32_t k, const uint32_t* mask,
+                           float* out_scores, int64_t* out_idx) {
+    B2_TRY(check_masked_args(idx, q, nq, q_dtype, k, mask));
+    if (nq == 0) return B2_OK;
+    if (!out_scores || !out_idx) { set_error("output buffers are NULL"); return B2_EINVAL; }
+    DeviceGuard guard(idx->device);
+    cudaStream_t st = idx->stream;
+    const size_t qbytes = (size_t)nq * idx->d * esize(q_dtype);
+    B2_TRY(idx->q_in.ensure(qbytes));
+    B2_TRY(idx->out_sc.ensure((size_t)nq * k * sizeof(float)));
+    B2_TRY(idx->out_id.ensure((size_t)nq * k * sizeof(int64_t)));
+    B2_CUDA(cudaMemcpyAsync(idx->q_in.p, q, qbytes, cudaMemcpyHostToDevice, st));
+    B2_TRY(upload_mask(idx, mask, st));
+    const void* q_dev = idx->q_in.p;
+    B2_TRY(adapt_queries(idx, q_dev, q_dtype, nq, st));
+    B2_TRY(masked_search(idx, q_dev, q_dtype, nq, k, idx->mask_dev.as<uint32_t>(), 0, idx->out_sc.as<float>(),
+                         idx->out_id.as<int64_t>(), st));
+    B2_CUDA(cudaMemcpyAsync(out_scores, idx->out_sc.p, (size_t)nq * k * sizeof(float), cudaMemcpyDeviceToHost, st));
+    B2_CUDA(cudaMemcpyAsync(out_idx, idx->out_id.p, (size_t)nq * k * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    cudaError_t e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) { set_error("masked search failed on the device: %s", cudaGetErrorString(e)); return B2_ECUDA; }
+    return B2_OK;
+}
+
 int b2_index_range_search(b2_index* idx, const void* q, int64_t nq, int32_t q_dtype, float radius, const int64_t* ids, int64_t n_ids,
                           int64_t* lims, float* out_d, int64_t* out_i, int64_t cap, int64_t* n_results) {
     if (!idx) { set_error("Index not loaded"); return B2_EINVAL; }
@@ -1373,13 +1463,20 @@ int b2_debug_filter_plan(int64_t nq, int64_t n, int32_t k, int32_t num_sms, int3
 
 // The raw candidate lists of one filter run on host queries, planned and launched exactly as search_core (level 0 / 1) or the
 // k-means assignment (top1) does it, so the tests can check the kernel's contract list by list instead of through finalize.
-int b2_debug_filter_lists(b2_index* idx, const void* q, int64_t nq, int32_t q_dtype, int32_t k, int32_t top1, int32_t level,
-                          int32_t* plan, float* rel_eps, float* cand_score, int32_t* cand_id, float* cand_thr) {
+// mask (host, nullable): the row bitmap of a masked search.
+static int debug_filter_lists(b2_index* idx, const void* q, int64_t nq, int32_t q_dtype, int32_t k, int32_t top1, int32_t level,
+                              const uint32_t* mask, int32_t* plan, float* rel_eps, float* cand_score, int32_t* cand_id,
+                              float* cand_thr) {
     B2_TRY(check_search_args(idx, q, nq, q_dtype, k));
     if (nq == 0 || !plan || !rel_eps || (level != 0 && level != 1)) { set_error("bad arguments"); return B2_EINVAL; }
     const bool lists = cand_score && cand_id && cand_thr;
     DeviceGuard guard(idx->device);
     cudaStream_t st = idx->stream;
+    const uint32_t* mask_dev = nullptr;
+    if (mask) {
+        B2_TRY(upload_mask(idx, mask, st));
+        mask_dev = idx->mask_dev.as<uint32_t>();
+    }
     if (idx->host) {
         // a host-resident index: the folded lists after the last corpus chunk, the one list of `cap` entries finalize reads,
         // reported as one split of two halves of cap / 2 (kp = cap) with its bound in both thr entries
@@ -1394,6 +1491,7 @@ int b2_debug_filter_lists(b2_index* idx, const void* q, int64_t nq, int32_t q_dt
         }
         FilterPlan p;
         B2_TRY(host_plan(idx, H, q_dev, q_dtype, nq, k, level, p));
+        p.X.mask = mask_dev;
         const int cap = p.use_filter ? finalize_capacity(p.kp, k) : 0;
         const FilterChunk c = p.use_filter ? p.chunks[0] : FilterChunk();
         plan[0] = cap ? 1 : 0;
@@ -1418,6 +1516,7 @@ int b2_debug_filter_lists(b2_index* idx, const void* q, int64_t nq, int32_t q_dt
         return B2_OK;
     }
     MatView X = idx->view;
+    X.mask = mask_dev;
     if (level == 1 || top1) X.filt16 = nullptr;  // the second level drops the bf16 copy; the k-means centroid view has none
     const size_t qbytes = (size_t)nq * idx->d * esize(q_dtype);
     const void* q_dev = nullptr;
@@ -1453,6 +1552,18 @@ int b2_debug_filter_lists(b2_index* idx, const void* q, int64_t nq, int32_t q_dt
     cudaError_t e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) { set_error("filter failed on the device: %s", cudaGetErrorString(e)); return B2_ECUDA; }
     return B2_OK;
+}
+
+int b2_debug_filter_lists(b2_index* idx, const void* q, int64_t nq, int32_t q_dtype, int32_t k, int32_t top1, int32_t level,
+                          int32_t* plan, float* rel_eps, float* cand_score, int32_t* cand_id, float* cand_thr) {
+    return debug_filter_lists(idx, q, nq, q_dtype, k, top1, level, nullptr, plan, rel_eps, cand_score, cand_id, cand_thr);
+}
+
+int b2_debug_filter_lists_masked(b2_index* idx, const void* q, int64_t nq, int32_t q_dtype, int32_t k, int32_t level,
+                                 const uint32_t* mask, int32_t* plan, float* rel_eps, float* cand_score, int32_t* cand_id,
+                                 float* cand_thr) {
+    if (idx && !mask && idx->n > 0) { set_error("mask is NULL"); return B2_EINVAL; }
+    return debug_filter_lists(idx, q, nq, q_dtype, k, 0, level, mask, plan, rel_eps, cand_score, cand_id, cand_thr);
 }
 
 // The chunking of a host-resident index (no device work): rows per chunk, chunks, ring slots.

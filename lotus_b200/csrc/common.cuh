@@ -153,6 +153,9 @@ struct MatView {
     float max_norm = 0.f;    // max_j ||x_j|| (upper bound), for the certification margin
     const float* max_norm_dev = nullptr;  // when set, the kernels read the bound from device memory instead (no host sync:
                                           // the k-means loop rebuilds its centroid view every iteration)
+    // masked search (optional): ceil(n / 32) words on the device, bit j & 31 of word j >> 5 set = row j takes part. The knn
+    // filter and the dense path leave the other rows out; null = every row. max_norm stays that of all rows (a looser bound).
+    const uint32_t* mask = nullptr;
 };
 
 // ---- kernels / launchers (one per .cu) ------------------------------------------------------------------

@@ -141,6 +141,7 @@ struct HostStore {
     size_t ring_bytes = 0;
     DevBuf slot[SLOTS], slot16[SLOTS];  // streamed rows as the filter reads them; int8 stores: their fp16 form for float queries
     DevBuf run_score, run_id, run_thr;  // running per-query lists of the fold
+    DevBuf mask_slice;  // masked search: the mask words of a chunk that does not start on a word boundary
     PinnedBuf staging_ids;
     cudaStream_t copy = nullptr;
     cudaEvent_t copied[SLOTS] = {}, freed[SLOTS] = {};
@@ -239,6 +240,7 @@ struct b2_index {
     } staged;
     DevBuf q_norm2;
     DevBuf q_wide;  // int8 queries on a floating-point store, widened exactly
+    DevBuf mask_dev;  // masked search from host buffers: the row bitmap of the call
     b2_index* f16_twin = nullptr;  // int8 indexes: the fp16 copy k-means runs on (kmeans_view)
     // host-resident indexes (b2_index_create_host): the rows live in pinned, mapped host memory and searches stream them
     // through a ring of device slots (host_resident.cu); `store` stays empty and `view.store` is the mapped pointer

@@ -612,10 +612,16 @@ __global__ void __launch_bounds__(128) fold_lists_kernel(const float* cand_score
 }
 
 // ---- dense exact path -----------------------------------------------------------------------------------------
+// A row mask (MatView::mask; null = every row) leaves the cleared rows out of the search: the selection kernels below behave
+// as if only the set rows existed, in their row order.
+__device__ __forceinline__ bool row_selected(const uint32_t* mask, int64_t j) {
+    return !mask || ((__ldg(mask + (j >> 5)) >> (j & 31)) & 1u) != 0;
+}
+
 // scores[s, j] = canonical score of selected query s against row j. One warp per row; the row's share stays
-// in registers/L1 while the warp walks the selected queries.
+// in registers/L1 while the warp walks the selected queries. A row the mask clears is not read: it gets the metric's worst value.
 __global__ void dense_scores_kernel(const void* store, int dtype, int64_t n, int d, const void* q, int q_dtype,
-                                    const int32_t* q_sel, int n_sel, int metric, float* out) {
+                                    const int32_t* q_sel, int n_sel, int metric, const uint32_t* mask, float* out) {
     extern __shared__ __align__(16) float dq[];  // [n_sel_chunk, d4] staged queries
     const int lane = threadIdx.x & 31;
     const int d4 = ((d + 3) >> 2) << 2;
@@ -635,6 +641,10 @@ __global__ void dense_scores_kernel(const void* store, int dtype, int64_t n, int
         }
         __syncthreads();
         for (int64_t j = warp; j < n; j += nwarps) {
+            if (!row_selected(mask, j)) {
+                if (lane < sc) out[(size_t)(s0 + lane) * n + j] = is_l2 ? FLT_MAX : -FLT_MAX;
+                continue;
+            }
             const char* row = reinterpret_cast<const char*>(store) + (size_t)j * d * esz;
             for (int s = 0; s < sc; ++s) {
                 const double part = is_l2 ? canonical_partial<true, true>(dq + s * d4, row, dtype, d, vec, lane)
@@ -670,7 +680,7 @@ __device__ __forceinline__ int block_excl_count(bool flag, int* s_warp, int& tot
 // One CTA per selected query: exact top-k of scores[s, 0..n) under faiss's heap rule.
 __global__ void __launch_bounds__(SEL_THREADS)
 dense_select_kernel(const float* scores, int64_t n, const int32_t* q_sel, int metric, int k, const int64_t* id_map,
-                    int64_t id_offset, float* out_scores, int64_t* out_idx) {
+                    int64_t id_offset, const uint32_t* mask, float* out_scores, int64_t* out_idx) {
     __shared__ int hist[256];
     __shared__ int s_warp[SEL_THREADS / 32];
     __shared__ uint32_t s_prefix, s_mask;
@@ -682,21 +692,37 @@ dense_select_kernel(const float* scores, int64_t n, const int32_t* q_sel, int me
     const float* row = scores + (size_t)s * n;
     const bool is_l2 = metric == B2_METRIC_L2;
     const int tid = threadIdx.x;
-    const int keff = (int)(n < k ? n : k);
+    // rows that take part: n, or the set bits of the mask (its bits at or past n are ignored)
+    int64_t m = n;
+    if (mask) {
+        int cnt = 0;
+        for (int64_t w = tid; w < (n + 31) >> 5; w += SEL_THREADS) {
+            uint32_t bits = __ldg(mask + w);
+            if (w == n >> 5) bits &= (1u << (n & 31)) - 1u;
+            cnt += __popc(bits);
+        }
+        if (tid == 0) s_nbetter = 0;
+        __syncthreads();
+        atomicAdd(&s_nbetter, cnt);
+        __syncthreads();
+        m = s_nbetter;
+        __syncthreads();
+    }
+    const int keff = (int)(m < k ? m : k);
 
     uint32_t vkey = 0xffffffffu;
     int r_keep = 0;
-    if (n > k) {
+    if (m > k) {
         // radix select: the k-th smallest best-first key
         if (tid == 0) { s_prefix = 0; s_mask = 0; s_kk = k; }
         __syncthreads();
         for (int shift = 24; shift >= 0; shift -= 8) {
             for (int i = tid; i < 256; i += SEL_THREADS) hist[i] = 0;
             __syncthreads();
-            const uint32_t prefix = s_prefix, mask = s_mask;
+            const uint32_t prefix = s_prefix, kmask = s_mask;
             for (int64_t j = tid; j < n; j += SEL_THREADS) {
                 const uint32_t key = best_first_key(row[j], metric);
-                if ((key & mask) == prefix) atomicAdd(&hist[(key >> shift) & 255], 1);
+                if ((key & kmask) == prefix && row_selected(mask, j)) atomicAdd(&hist[(key >> shift) & 255], 1);
             }
             __syncthreads();
             if (tid == 0) {
@@ -707,7 +733,7 @@ dense_select_kernel(const float* scores, int64_t n, const int32_t* q_sel, int me
                 }
                 s_kk = kk - cum;
                 s_prefix = prefix | ((uint32_t)b << shift);
-                s_mask = mask | (0xffu << shift);
+                s_mask = kmask | (0xffu << shift);
             }
             __syncthreads();
         }
@@ -723,9 +749,9 @@ dense_select_kernel(const float* scores, int64_t n, const int32_t* q_sel, int me
         const int64_t j = base + tid;
         uint32_t key = 0xffffffffu;
         bool in_s = false, is_tie = false, better = false;
-        if (j < n) {
+        if (j < n && row_selected(mask, j)) {
             key = best_first_key(row[j], metric);
-            if (n > k) {
+            if (m > k) {
                 better = key < vkey;
                 is_tie = key == vkey;
                 in_s = better || is_tie;
@@ -738,7 +764,7 @@ dense_select_kernel(const float* scores, int64_t n, const int32_t* q_sel, int me
             const uint32_t tie = is_l2 ? (uint32_t)j : ~(uint32_t)j;
             if (slot < SEL_MAX_K) s_out[slot] = ((uint64_t)key << 32) | tie;
         }
-        if (n > k && running_s < k) {  // running_s is block-uniform
+        if (m > k && running_s < k) {  // running_s is block-uniform
             if (__syncthreads_or(in_s)) {
                 int tot_s = 0;
                 const int pos = running_s + block_excl_count(in_s, s_warp, tot_s);
@@ -756,7 +782,7 @@ dense_select_kernel(const float* scores, int64_t n, const int32_t* q_sel, int me
     }
     __syncthreads();
     const int c = s_nbetter;
-    if (n > k) {
+    if (m > k) {
         const int t = s_nties;
         // L2: first r ties (ascending id). IP: the last r of the t window ties (e_{t-r+1} .. e_t).
         const int first = is_l2 ? 0 : t - r_keep;
@@ -806,17 +832,20 @@ dense_select_kernel(const float* scores, int64_t n, const int32_t* q_sel, int me
 // by a device-wide radix sort (CUB — library code, a plumbing step here: the scores are ours), and the first k are unpacked.
 // faiss switches to a reservoir for k >= 100 whose tie retention at the cut is unspecified; sorted truncation with the heap's
 // order ((score desc, id desc) for IP, (dist asc, id asc) for L2) is used.
-__global__ void dense_keys_kernel(const float* scores, int64_t n, int rows, int metric, uint64_t* keys) {
+__global__ void dense_keys_kernel(const float* scores, int64_t n, int rows, int metric, const uint32_t* mask, uint64_t* keys) {
     const bool is_l2 = metric == B2_METRIC_L2;
     const int64_t total = (int64_t)rows * n;
     for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
         const int64_t j = t % n;
-        keys[t] = ((uint64_t)best_first_key(scores[t], metric) << 32) | (is_l2 ? (uint32_t)j : ~(uint32_t)j);
+        // a row the mask clears sorts behind every row that takes part; dense_unpack_kernel reports none of them
+        const uint32_t key = row_selected(mask, j) ? best_first_key(scores[t], metric) : 0xffffffffu;
+        keys[t] = ((uint64_t)key << 32) | (is_l2 ? (uint32_t)j : ~(uint32_t)j);
     }
 }
 
 __global__ void dense_unpack_kernel(const uint64_t* keys, int64_t n, int rows, const int32_t* q_sel, int64_t q_base, int metric, int k,
-                                    const int64_t* id_map, int64_t id_offset, float* out_scores, int64_t* out_idx) {
+                                    const int64_t* id_map, int64_t id_offset, const uint32_t* mask, float* out_scores,
+                                    int64_t* out_idx) {
     const bool is_l2 = metric == B2_METRIC_L2;
     const float pad = is_l2 ? FLT_MAX : -FLT_MAX;
     const int64_t total = (int64_t)rows * k;
@@ -829,8 +858,10 @@ __global__ void dense_unpack_kernel(const uint64_t* keys, int64_t n, int rows, c
             const uint64_t e = keys[s * n + o];
             const uint32_t lo = (uint32_t)(e & 0xffffffffu);
             const int64_t id = (int64_t)(is_l2 ? lo : ~lo);
-            sc = best_first_unkey((uint32_t)(e >> 32), metric);
-            oid = id_map ? id_map[id] : id + id_offset;
+            if (row_selected(mask, id)) {
+                sc = best_first_unkey((uint32_t)(e >> 32), metric);
+                oid = id_map ? id_map[id] : id + id_offset;
+            }
         }
         out_scores[(size_t)qo * k + o] = sc;
         out_idx[(size_t)qo * k + o] = oid;
@@ -1199,7 +1230,7 @@ int launch_dense_topk(const MatView& X, const void* q, int q_dtype, int64_t nq, 
         const void* qb = q_sel ? q : reinterpret_cast<const char*>(q) + (size_t)s0 * X.d * esize(q_dtype);
         if (X.n > 0) {
             dense_scores_kernel<<<grid_for(X.n * 32, 256, 132 * 8), 256, smem, stream>>>(X.store, X.dtype, X.n, X.d, qb, q_dtype,
-                                                                                       sel, sc, metric, dense_ws);
+                                                                                       sel, sc, metric, X.mask, dense_ws);
             B2_LAUNCH_CHECK();
         }
         if (full_sort) {
@@ -1209,7 +1240,7 @@ int launch_dense_topk(const MatView& X, const void* q, int q_dtype, int64_t nq, 
             void* temp = k_out + (size_t)dense_ws_rows * X.n;
             size_t temp_bytes = dense_sort_ws_bytes(dense_ws_rows, X.n) - 2 * (size_t)dense_ws_rows * X.n * sizeof(uint64_t) - 512;
             if (X.n > 0) {
-                dense_keys_kernel<<<grid_for((int64_t)items, 256), 256, 0, stream>>>(dense_ws, X.n, sc, metric, k_in);
+                dense_keys_kernel<<<grid_for((int64_t)items, 256), 256, 0, stream>>>(dense_ws, X.n, sc, metric, X.mask, k_in);
                 B2_LAUNCH_CHECK();
                 if (dense_ws_rows <= 4) {
                     for (int r = 0; r < sc; ++r)
@@ -1223,12 +1254,12 @@ int launch_dense_topk(const MatView& X, const void* q, int q_dtype, int64_t nq, 
                 g_stats[ST_LAUNCHES]++;
             }
             dense_unpack_kernel<<<grid_for((int64_t)sc * k, 256), 256, 0, stream>>>(k_out, X.n, sc, sel, s0, metric, k, id_map, id_offset,
-                                                                                  out_scores, out_idx);
+                                                                                  X.mask, out_scores, out_idx);
             B2_LAUNCH_CHECK();
         } else {
             float* os = q_sel ? out_scores : out_scores + (size_t)s0 * k;
             int64_t* oi = q_sel ? out_idx : out_idx + (size_t)s0 * k;
-            dense_select_kernel<<<sc, SEL_THREADS, 0, stream>>>(dense_ws, X.n, sel, metric, k, id_map, id_offset, os, oi);
+            dense_select_kernel<<<sc, SEL_THREADS, 0, stream>>>(dense_ws, X.n, sel, metric, k, id_map, id_offset, X.mask, os, oi);
             B2_LAUNCH_CHECK();
         }
     }

@@ -626,6 +626,19 @@ __device__ __forceinline__ void prepare8(float (&v)[8], int idx0, int valid, con
     }
 }
 
+// The same under a row mask: bit j of `live` set = column j is a selected row of the corpus; the others can enter no list
+template <bool IS_L2>
+__device__ __forceinline__ void prepare8_masked(float (&v)[8], int idx0, uint32_t live, const float* xnorm) {
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        if ((live >> j) & 1u) {
+            if constexpr (IS_L2) v[j] = fmaf(2.f, v[j], -__ldg(xnorm + idx0 + j));
+        } else {
+            v[j] = -INFINITY;
+        }
+    }
+}
+
 // Eight consecutive scores of the lane's (row, set), in a chunk where some lane of the warp beats its threshold (the
 // consumer's gate skips the others): 8 branch-free predicated appends into the pending buffer and one vote on a flush.
 // The pending buffers are merged into the lists by the whole warp in lockstep once any lane holds PEND_FLUSH candidates.
@@ -677,15 +690,26 @@ __device__ __forceinline__ int32_t i8_score(int32_t s, const FilterParams& p, in
     else return s;
 }
 
-template <int KP, bool IS_L2, Op OP, int CL, bool TOP1>
-__device__ __forceinline__ void knn_filter_body(const CUtensorMap& tmap_q, const CUtensorMap& tmap_x, const FilterParams& p) {
+//
+// MASKED: only the corpus rows whose bit is set in `mask` (bit j & 31 of word j >> 5 is row j) take part. The eight words of a
+// corpus tile are the same for every query row: lane l of each consumer warp loads word l & 7 before the tile's wgmmas are
+// issued and holds it across them; the epilogue fetches a chunk's word with a shuffle. A chunk whose 16 bits are clear is
+// skipped outright, a tile whose 256 bits are clear skips its epilogue (its stages are consumed all the same: the producer
+// does not look at the mask), and a cleared column reaches neither the gate nor the lists. So `thr` still bounds every
+// SELECTED row a list discarded, which is all the certificate asks of it.
+template <int KP, bool IS_L2, Op OP, int CL, bool TOP1, bool MASKED = false>
+__device__ __forceinline__ void knn_filter_body(const CUtensorMap& tmap_q, const CUtensorMap& tmap_x, const FilterParams& p,
+                                                const uint32_t* mask = nullptr) {
+    static_assert(!(TOP1 && MASKED), "the k-means top-2 epilogue takes no row mask");
     using AccT = std::conditional_t<OP == Op::I8, int32_t, float>;
     constexpr int NSTAGES = num_stages(KP);
     static_assert(NSTAGES >= 2, "not enough shared memory for the operand ring");
     constexpr int KPH = KP / 2;  // candidates kept per (row, set)
     static_assert(KPH % 4 == 0, "list length must allow float4 write-out");
     constexpr int LSET = list_set_stride(KPH);
-    constexpr int RES_KB = FILTER_RES_KB;
+    // the masked epilogue's bit tests need a few registers more than the column-range compares they replace (the L2 forms
+    // spilled two): a masked kernel keeps one query K-block fewer in registers
+    constexpr int RES_KB = MASKED ? FILTER_RES_KB - 1 : FILTER_RES_KB;
 
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = align_smem(smem_raw);
@@ -742,11 +766,29 @@ __device__ __forceinline__ void knn_filter_body(const CUtensorMap& tmap_q, const
             // int8: gthr rounded down (an integer score s beats t exactly when s > floor(t); -inf maps to INT_MIN)
             int32_t gthr_i[2][2] = {{INT_MIN, INT_MIN}, {INT_MIN, INT_MIN}};
             for (int t = t0; t < t1; ++t) {
+                if constexpr (MASKED) {  // the tile's 32 bytes of mask, on their way while the wgmmas run
+                    if (lane == 0) asm volatile("prefetch.global.L1 [%0];" ::"l"(mask + t * (BLOCK_N / 32)));
+                }
                 mma_tile<OP, NSTAGES, CL, RES_KB>(acc, afrag, t == t0, ring, p.num_kb, g, sc.cta, stage, phase);
                 const int col0 = t * BLOCK_N;
                 const int ncols = min(BLOCK_N, p.n - col0);
+                uint32_t mword = 0;  // MASKED: word (lane & 7) of the tile's mask, zero past the last word of the corpus
+                if constexpr (MASKED) {
+                    const int w = t * (BLOCK_N / 32) + (lane & 7);
+                    if (w < (p.n + 31) >> 5) mword = __ldg(mask + w);
+                    if (!__any_sync(0xffffffffu, mword != 0)) continue;  // no selected row in this tile
+                }
 #pragma unroll
                 for (int c = 0; c < BLOCK_N / 16; ++c) {  // 16-column chunks through the per-warp transpose
+                    // MASKED: bit i set = column 16 c + i is a selected row of the corpus; it stands in for the column-range
+                    // tests of the unmasked epilogue, so the mask adds no compare to a chunk
+                    uint32_t live = 0xffffu;
+                    if constexpr (MASKED) {
+                        live = (__shfl_sync(0xffffffffu, mword, c >> 1) >> (16 * (c & 1))) & 0xffffu;
+                        const int rem = ncols - 16 * c;
+                        if (rem < 16) live &= rem > 0 ? (1u << rem) - 1u : 0u;
+                        if (live == 0) continue;  // warp-uniform: nothing selected in this chunk
+                    }
                     if constexpr (!TOP1) {
                         // Gate: test the chunk's fragment values, as prepare8 transforms them, against the thresholds of
                         // their lists. When no lane holds a value above its threshold (late in a sweep almost always),
@@ -757,15 +799,17 @@ __device__ __forceinline__ void knn_filter_body(const CUtensorMap& tmap_q, const
 #pragma unroll
                             for (int h = 0; h < 4; ++h) {  // acc[a + h]: row fr + 8 (h >> 1), column 16c + 8jj + fc + (h & 1)
                                 const int off = 16 * c + 8 * jj + fc + (h & 1);
+                                bool in;
+                                if constexpr (MASKED) in = ((live >> (8 * jj + (h & 1))) >> fc & 1u) != 0;
+                                else in = off < ncols;
                                 if constexpr (OP == Op::I8) {
-                                    hit |= off < ncols && i8_score<IS_L2>(acc[(2 * c + jj) * 4 + h], p, col0 + off, off < ncols) >
-                                                              gthr_i[h >> 1][jj];
+                                    hit |= in && i8_score<IS_L2>(acc[(2 * c + jj) * 4 + h], p, col0 + off, in) > gthr_i[h >> 1][jj];
                                 } else {
                                     float s = (float)acc[(2 * c + jj) * 4 + h];
                                     if constexpr (IS_L2) {
-                                        if (off < ncols) s = fmaf(2.f, s, -__ldg(p.xnorm + col0 + off));
+                                        if (in) s = fmaf(2.f, s, -__ldg(p.xnorm + col0 + off));
                                     }
-                                    hit |= off < ncols && s > gthr[h >> 1][jj];
+                                    hit |= in && s > gthr[h >> 1][jj];
                                 }
                             }
                         }
@@ -793,7 +837,8 @@ __device__ __forceinline__ void knn_filter_body(const CUtensorMap& tmap_q, const
 #pragma unroll
                     for (int j = 0; j < 8; ++j) v[j] = xs[rr * XP_STRIDE + 8 * e + j];
                     const int off = 16 * c + 8 * e;
-                    prepare8<IS_L2 && OP != Op::I8>(v, col0 + off, ncols - off, p.xnorm);  // int8: transformed already
+                    if constexpr (MASKED) prepare8_masked<IS_L2 && OP != Op::I8>(v, col0 + off, live >> (8 * e), p.xnorm);
+                    else prepare8<IS_L2 && OP != Op::I8>(v, col0 + off, ncols - off, p.xnorm);  // int8: transformed already
                     if constexpr (TOP1) {
                         process8_top2(v, col0 + off, b1, b2, b3, i1, i2);
                     } else {
@@ -866,6 +911,22 @@ __global__ void __launch_bounds__(NUM_THREADS, 1)
 knn_i8_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_x,
                      const FilterParams p) {
     knn_filter_body<KP, IS_L2, Op::I8, CL, false>(tmap_q, tmap_x, p);
+}
+
+// the masked knn filter (masked search): entries of their own, so that the kernels of an unmasked search are untouched.
+// mask: ceil(p.n / 32) words, see knn_filter_body
+template <int KP, bool IS_L2, Op OP, int CL>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+knn_masked_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_x,
+                         const FilterParams p, const uint32_t* __restrict__ mask) {
+    knn_filter_body<KP, IS_L2, OP, CL, false, true>(tmap_q, tmap_x, p, mask);
+}
+
+template <int KP, bool IS_L2, int CL>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+knn_masked_i8_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_x,
+                            const FilterParams p, const uint32_t* __restrict__ mask) {
+    knn_filter_body<KP, IS_L2, Op::I8, CL, false, true>(tmap_q, tmap_x, p, mask);
 }
 
 // ---- all-pairs threshold filter (sem_dedup): same mainloop, the epilogue emits (i, j) candidates -------------------
@@ -1117,9 +1178,9 @@ int make_tmap(CUtensorMap* map, const void* base, Op op, int64_t rows, int64_t c
     return B2_OK;
 }
 
-template <typename Kern>
+template <typename Kern, typename... Extra>
 int launch_cluster(Kern kern, int grid, int smem, int cl, const CUtensorMap& tq, const CUtensorMap& tx, const FilterParams& p,
-                   cudaStream_t stream) {
+                   cudaStream_t stream, Extra... extra) {
     // the attribute is per DEVICE (not per process): set it on every launch — a microsecond — so that a process driving
     // several GPUs (B200VS(device=i) for several i) launches correctly on each of them
     B2_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
@@ -1135,7 +1196,7 @@ int launch_cluster(Kern kern, int grid, int smem, int cl, const CUtensorMap& tq,
     attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    B2_CUDA(cudaLaunchKernelEx(&cfg, kern, tq, tx, p));
+    B2_CUDA(cudaLaunchKernelEx(&cfg, kern, tq, tx, p, extra...));
     B2_LAUNCH_CHECK();
     g_stats[ST_FILTER_LAUNCHES]++;
     return B2_OK;
@@ -1144,6 +1205,19 @@ int launch_cluster(Kern kern, int grid, int smem, int cl, const CUtensorMap& tq,
 template <int KP, bool IS_L2, Op OP, int CL, bool TOP1 = false>
 int launch_variant(const CUtensorMap& tq, const CUtensorMap& tx, const FilterParams& p, int grid, cudaStream_t stream) {
     return launch_cluster(knn_filter_kernel<KP, IS_L2, OP, CL, TOP1>, grid, smem_bytes(KP), CL, tq, tx, p, stream);
+}
+
+// the masked kernels (mask != nullptr): same grid, shared memory and schedule as the unmasked ones
+template <int KP, bool IS_L2, int CL>
+int launch_masked_op(Op op, const CUtensorMap& tq, const CUtensorMap& tx, const FilterParams& p, int grid, const uint32_t* mask,
+                     cudaStream_t stream) {
+    constexpr int SMEM = smem_bytes(KP);
+    switch (op) {
+        case Op::TF32: return launch_cluster(knn_masked_filter_kernel<KP, IS_L2, Op::TF32, CL>, grid, SMEM, CL, tq, tx, p, stream, mask);
+        case Op::BF16: return launch_cluster(knn_masked_filter_kernel<KP, IS_L2, Op::BF16, CL>, grid, SMEM, CL, tq, tx, p, stream, mask);
+        case Op::I8: return launch_cluster(knn_masked_i8_filter_kernel<KP, IS_L2, CL>, grid, SMEM, CL, tq, tx, p, stream, mask);
+        default: return launch_cluster(knn_masked_filter_kernel<KP, IS_L2, Op::F16, CL>, grid, SMEM, CL, tq, tx, p, stream, mask);  // Op::F16
+    }
 }
 
 template <int KP, bool IS_L2, int CL, bool TOP1 = false>
@@ -1164,7 +1238,10 @@ int launch_op(Op op, const CUtensorMap& tq, const CUtensorMap& tx, const FilterP
 
 template <int KP, int CL>
 int launch_kp(bool is_l2, Op op, const CUtensorMap& tq, const CUtensorMap& tx, const FilterParams& p, int grid,
-              cudaStream_t stream) {
+              const uint32_t* mask, cudaStream_t stream) {
+    if (mask)
+        return is_l2 ? launch_masked_op<KP, true, CL>(op, tq, tx, p, grid, mask, stream)
+                     : launch_masked_op<KP, false, CL>(op, tq, tx, p, grid, mask, stream);
     return is_l2 ? launch_op<KP, true, CL>(op, tq, tx, p, grid, stream) : launch_op<KP, false, CL>(op, tq, tx, p, grid, stream);
 }
 
@@ -1178,12 +1255,12 @@ int launch_top1(bool is_l2, Op op, const CUtensorMap& tq, const CUtensorMap& tx,
 
 template <int CL>
 int launch_cl(int kp, bool is_l2, Op op, const CUtensorMap& tq, const CUtensorMap& tx, const FilterParams& p, int grid,
-              cudaStream_t stream) {
+              const uint32_t* mask, cudaStream_t stream) {
     switch (kp) {
-        case 16: return launch_kp<16, CL>(is_l2, op, tq, tx, p, grid, stream);
-        case 32: return launch_kp<32, CL>(is_l2, op, tq, tx, p, grid, stream);
-        case 64: return launch_kp<64, CL>(is_l2, op, tq, tx, p, grid, stream);
-        case 72: return launch_kp<72, CL>(is_l2, op, tq, tx, p, grid, stream);
+        case 16: return launch_kp<16, CL>(is_l2, op, tq, tx, p, grid, mask, stream);
+        case 32: return launch_kp<32, CL>(is_l2, op, tq, tx, p, grid, mask, stream);
+        case 64: return launch_kp<64, CL>(is_l2, op, tq, tx, p, grid, mask, stream);
+        case 72: return launch_kp<72, CL>(is_l2, op, tq, tx, p, grid, mask, stream);
         default: set_error("internal: unsupported candidate capacity %d", kp); return B2_EINVAL;
     }
 }
@@ -1413,12 +1490,17 @@ int launch_knn_filter(const MatView& X, const void* q_filt, int64_t q_pitch, int
     }
     // workers are CTA pairs in cluster mode; in clusters of four both counts are even, so whole clusters are launched
     const int grid = (cluster > 1 ? 2 : 1) * (int)std::min<int64_t>(items, workers);
-    if (p.top1)
+    if (p.top1) {
+        if (X.mask) {
+            set_error("internal: the k-means assignment takes no row mask");
+            return B2_EINVAL;
+        }
         return cluster == 1 ? launch_top1<1>(is_l2, op, tq, tx, p, grid, stream) : launch_top1<2>(is_l2, op, tq, tx, p, grid, stream);
+    }
     switch (cluster) {
-        case 1: return launch_cl<1>(kp, is_l2, op, tq, tx, p, grid, stream);
-        case 2: return launch_cl<2>(kp, is_l2, op, tq, tx, p, grid, stream);
-        default: return launch_cl<FILTER_CL>(kp, is_l2, op, tq, tx, p, grid, stream);
+        case 1: return launch_cl<1>(kp, is_l2, op, tq, tx, p, grid, X.mask, stream);
+        case 2: return launch_cl<2>(kp, is_l2, op, tq, tx, p, grid, X.mask, stream);
+        default: return launch_cl<FILTER_CL>(kp, is_l2, op, tq, tx, p, grid, X.mask, stream);
     }
 }
 

@@ -210,6 +210,18 @@ class MultiDeviceIndex:
         parts = list(self.pool.map(one, range(len(self.shards))))
         return merge_shard_lists([p[0] for p in parts], [p[1] for p in parts], self.metric)
 
+    def search_masked(self, q: np.ndarray, k: int, q_dtype: int, mask):
+        """As `_native.Index.search_masked`: every shard searches its rows under its slice of the bitmap (built on the host:
+        shard bounds need not fall on word boundaries)."""
+        words = nv.pack_mask(mask, self.n)
+
+        def one(g):
+            lo, hi = self.bounds[g]
+            D, I = self.shards[g].search_masked(q, k, q_dtype, nv.slice_mask(words, self.n, lo, hi))
+            return D, np.where(I >= 0, I + lo, -1)
+        parts = list(self.pool.map(one, range(len(self.shards))))
+        return merge_shard_lists([p[0] for p in parts], [p[1] for p in parts], self.metric)
+
     def range_search(self, q: np.ndarray, radius: float, q_dtype: int = nv.F32, ids: np.ndarray | None = None):
         """(lims, D, I) as `_native.Index.range_search`. Each shard answers for its rows (an ids subset: the distinct ids it
         holds); the hits are then ordered per query by row id, or with ids by position in `ids`, where a repeated id
@@ -319,6 +331,15 @@ def device_footprint(n: int, d: int, code: int) -> int:
     return total + n * (8 if code == nv.I8 else 4)
 
 
+def ring_row_bytes(d: int, code: int) -> int:
+    """Device bytes one streamed row of a host-resident index takes in its ring (the filter-ready row, plus its fp16 form for
+    an int8 store): mirrors ring_row_bytes in api.cu."""
+    esz = {nv.F32: 4, nv.BF16: 2, nv.F16: 2, nv.I8: 1}[code]
+    align = 16 // esz
+    b = -(-d // align) * align * esz
+    return b + (-(-d // 8) * 8 * 2 if code == nv.I8 else 0)
+
+
 AUTO_MARGIN = 1 << 30  # residency="auto": device memory left free beyond the footprint, for search workspaces
 
 
@@ -332,21 +353,36 @@ class B200VS(VS):
     upcast of the stored values), "i8" (store int8: embeddings whose values are all integers in [-128, 127], such as
     quantized embeddings, of any numeric type; anything else raises ValueError, as the store never picks a scale. int8 queries
     are searched on the int8 tensor cores, floating-point queries against an fp16 copy of the rows made on their first
-    search; results equal faiss on the float32 upcast; dedup and k-means are not available), or "auto" (bf16 only when
-    handed a bf16 tensor, float32 otherwise; int8 input still gives a float32 store).
+    search; results equal faiss on the float32 upcast; dedup runs the int8 pair filter, with its threshold in units of int8
+    inner products, and k-means an fp16 copy of the rows), or "auto" (bf16 only when handed a bf16 tensor, float32 otherwise;
+    int8 input still gives a float32 store).
     residency: "device" (default: the rows live in device memory), "host" (the rows stay in pinned host memory and every
     search streams them through a device ring of ring_bytes, None = the library default: corpora larger than free device
     memory, same results bit for bit; threshold_pairs / kmeans, hence sem_dedup / sem_cluster_by, raise ValueError) or
     "auto" (device when the store's device footprint plus a 1 GiB margin fits in free device memory, host otherwise;
     `resident(index_dir)` reports the choice). CUDA tensors given to a host-resident store are copied to the host.
+    subset: how `__call__(..., ids=...)` searches a subset of the rows. "gather" (default): a temporary index over a gathered
+    copy of vecs[ids], as the reference does. "mask": when ids is strictly ascending (what a pandas filter leaves) the whole
+    index is swept under a row bitmap instead, with the same result bit for bit, no copy of the subset in device memory and,
+    on a host-resident index, no gather on the host; any other ids (permuted or repeating: different tie order) take the
+    gathered path. "auto": the bitmap, for a strictly ascending ids, where the gathered copy is what hurts: on a
+    host-resident index when the subset does not fit its ring (it would be gathered on the host), on a device-resident one
+    when the copy's footprint plus a 1 GiB margin does not fit in free device memory (the gathered search would fail with
+    an allocation error). Everywhere else the gathered search was the faster one in bench_masked.py (H100 80GB HBM3 at a
+    700 W power limit, 1M x 768, subsets of 90 % down to 1 % of the rows: a masked search sweeps every row whatever the
+    subset's size), so "auto" keeps it there; on the host-resident index the bitmap won for the subsets of 90 % and 50 %,
+    the ones larger than its 384 MB ring.
     """
 
     accepts_id_arrays = True  # `ids=` may be a numpy int64 array (the operators then skip building a Python list)
 
     def __init__(self, factory_string: str = "Flat", metric: int = METRIC_INNER_PRODUCT, dtype: str = "auto",
                  device: int = 0, cache_size: int = 4, devices: "list[int] | None" = None, residency: str = "device",
-                 ring_bytes: "int | None" = None):
+                 ring_bytes: "int | None" = None, subset: str = "gather"):
         super().__init__()
+        if subset not in ("gather", "mask", "auto"):
+            raise ValueError("subset must be 'gather', 'mask' or 'auto'")
+        self.subset = subset
         if residency not in ("device", "host", "auto"):
             raise ValueError("residency must be 'device', 'host' or 'auto'")
         if ring_bytes is not None and (not isinstance(ring_bytes, int) or ring_bytes < 0):
@@ -514,7 +550,38 @@ class B200VS(VS):
         if q.shape[1] != self.b2_index.d:
             raise ValueError(f"query dimension {q.shape[1]} does not match the index dimension {self.b2_index.d}")
         try:
-            distances, indices = self.b2_index.search(q, int(K), code, ids=ids_a)
+            if ids_a is not None and self._subset_by_mask(ids_a):
+                distances, indices = self.b2_index.search_masked(q, int(K), code, nv.ids_to_mask(ids_a, self.b2_index.n))
+            else:
+                distances, indices = self.b2_index.search(q, int(K), code, ids=ids_a)
+        except nv.NativeError as e:
+            if e.code in (nv.EINVAL, nv.ERANGE):
+                raise ValueError(e.msg) from e
+            raise
+        return RMOutput(distances=distances, indices=indices)
+
+    def _subset_by_mask(self, ids: np.ndarray) -> bool:
+        """Whether `subset` sends this ids subset through the masked search (see the class docstring)."""
+        idx = self.b2_index
+        if self.subset == "gather" or len(ids) == 0 or not nv.strictly_ascending(ids):
+            return False
+        if self.subset == "mask":
+            return True
+        if getattr(idx, "resident", "device") == "host":
+            return len(ids) * ring_row_bytes(idx.d, idx.dtype) > idx.ring_bytes
+        return device_footprint(len(ids), idx.d, idx.dtype) + AUTO_MARGIN > _free_device_bytes(idx.device)
+
+    def search_masked(self, query_vectors: Any, K: int, mask: Any) -> RMOutput:
+        """__call__(query_vectors, K, ids=np.flatnonzero(mask)) for callers that hold a boolean column rather than ids: the
+        rows whose entry of `mask` (bool, one per row of the index) is set, always searched under the bitmap."""
+        if self.b2_index is None or self.index_dir is None:
+            raise ValueError("Index not loaded")
+        q, code, _ = _to_host_matrix(query_vectors, False, exact_bf16_ok=self.b2_index.dtype == nv.BF16, scratch=self._scratch,
+                                     pass_f16=True, pass_i8=True)
+        if q.shape[1] != self.b2_index.d:
+            raise ValueError(f"query dimension {q.shape[1]} does not match the index dimension {self.b2_index.d}")
+        try:
+            distances, indices = self.b2_index.search_masked(q, int(K), code, np.asarray(mask, dtype=np.bool_))
         except nv.NativeError as e:
             if e.code in (nv.EINVAL, nv.ERANGE):
                 raise ValueError(e.msg) from e
