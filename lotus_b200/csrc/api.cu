@@ -237,117 +237,25 @@ int run_filter(b2_index* idx, const FilterPlan& p, const FilterChunk& c, int met
     return B2_OK;
 }
 
+// The candidate lists finalize reads for one query chunk: per query n_lists lists of list_len entries, each with its bound in
+// thr. The filter leaves 2 * n_splits lists of kp / 2 (two epilogue sets per split); a streamed search folds the lists of every
+// corpus chunk into one list of finalize_capacity(kp, k) entries.
+struct CandLists {
+    const float* score;
+    const int32_t* id;
+    const float* thr;
+    int list_len, n_lists;
+};
+
+// the lists run_filter left for chunk c
+static CandLists filter_lists(b2_index* idx, const FilterPlan& p, const FilterChunk& c) {
+    return {idx->cand_score.as<float>(), idx->cand_id.as<int32_t>(), idx->cand_thr.as<float>(), p.kp / 2, 2 * c.n_splits};
+}
+
 // rows of the dense path's score workspace (score row of 4 bytes per column, plus two sort-key buffers on the full-sort path)
 // within 512 MB
 static int64_t dense_rows_cap(int64_t n, bool full_sort) {
     return std::max<int64_t>(1, (int64_t)(512ull << 20) / (std::max<int64_t>(n, 1) * (full_sort ? 24 : 4)));
-}
-
-// Finalize/certify the candidate lists run_filter left for chunk c (hint: a lower bound the k-th score is known to reach, or
-// null), read the one counter back and add the filter's event time to idx->last_filter_ms. The queries the certificate leaves
-// open are compacted into idx->sel[1 .. 1 + *n_open]; with `fallback` the exact dense path answers them here.
-static int certify(b2_index* idx, const FilterPlan& p, const FilterChunk& c, int metric, const int64_t* id_map, int64_t id_offset,
-                   float* out_sc, int64_t* out_id, const float* hint, bool fallback, int64_t* n_open, cudaStream_t st) {
-    const MatView& X = p.X;
-    const void* qc = reinterpret_cast<const char*>(p.q) + (size_t)c.q0 * X.d * esize(p.q_dtype);
-    float* osc = out_sc + (size_t)c.q0 * p.k;
-    int64_t* oid = out_id + (size_t)c.q0 * p.k;
-    B2_TRY(idx->flags.ensure((size_t)c.nq * sizeof(int32_t)));
-    B2_TRY(idx->sel.ensure((size_t)(c.nq + 1) * sizeof(int32_t)));  // [0] = counter, [1..] = uncertified queries
-    B2_TRY(idx->h_flags.ensure(64));
-    int32_t* sel_count = idx->sel.as<int32_t>();
-    int32_t* sel_list = sel_count + 1;
-    B2_CUDA(cudaMemsetAsync(sel_count, 0, sizeof(int32_t), st));
-    B2_TRY(launch_finalize(X, qc, p.q_dtype, c.nq, metric, p.k, p.kp, p.kp / 2, 2 * c.n_splits, idx->cand_score.as<float>(),
-                           idx->cand_id.as<int32_t>(), idx->cand_thr.as<float>(), p.rel_eps, p.abs_eps, p.q_norm_limit, id_map, id_offset, osc, oid,
-                           idx->flags.as<int32_t>(), sel_list, sel_count, st, hint));
-    // the certificate outcome comes back as ONE counter (the failed queries are compacted on the device)
-    int32_t* h_count = reinterpret_cast<int32_t*>(idx->h_flags.p);
-    B2_CUDA(cudaMemcpyAsync(h_count, sel_count, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-    cudaError_t se = cudaStreamSynchronize(st);
-    if (se != cudaSuccess) {
-        set_error("search pipeline failed on the device: %s", cudaGetErrorString(se));
-        return B2_ECUDA;
-    }
-    float ms = -1.f;
-    if (cudaEventElapsedTime(&ms, idx->ev0, idx->ev1) == cudaSuccess)
-        idx->last_filter_ms = (idx->last_filter_ms < 0 ? 0.f : idx->last_filter_ms) + ms;
-    const int64_t n_sel = *h_count;
-    *n_open = n_sel;
-    if (!fallback || n_sel == 0) return B2_OK;
-    // exact fallback for the queries the certificate could not cover
-    if (p.k > dense_max_k()) {
-        set_error("internal: fallback with k=%d", p.k);
-        return B2_ERANGE;
-    }
-    g_stats[ST_FALLBACK] += n_sel;
-    const int64_t rows = std::min<int64_t>(dense_rows_cap(X.n, false), n_sel);
-    B2_TRY(idx->dense.ensure((size_t)rows * X.n * sizeof(float)));
-    return launch_dense_topk(X, qc, p.q_dtype, c.nq, sel_list, n_sel, metric, p.k, id_map, id_offset, idx->dense.as<float>(), rows,
-                             nullptr, osc, oid, st);
-}
-
-// level 0: the caller's search. On a two-level plan the queries whose first-level certificate fails are deferred, gathered and
-// answered by a level-1 call (tf32 filter on the same store, then the dense path for what still fails) and scattered back.
-int search_core(b2_index* idx, const MatView& X_in, int metric, const void* q_dev, int q_dtype, int64_t nq, int k,
-                       const int64_t* id_map, int64_t id_offset, float* out_sc, int64_t* out_id, cudaStream_t st, int level) {
-    if (level == 0) idx->last_filter_ms = -1.f;
-    if (nq <= 0) return B2_OK;
-    if (level == 0) g_stats[ST_QUERIES] += nq;
-    if (X_in.n <= 0) {
-        fill_pad_kernel<<<132, 256, 0, st>>>(out_sc, out_id, nq * k, metric == B2_METRIC_L2 ? FLT_MAX : -FLT_MAX);
-        B2_LAUNCH_CHECK();
-        return B2_OK;
-    }
-    FilterPlan p;
-    B2_TRY(plan_filter(X_in, q_dev, q_dtype, nq, k, false, idx->device, p));
-    const MatView& X = p.X;
-    if (!p.use_filter) {
-        if (k > dense_max_k()) {
-            set_error("k=%d is not supported (max %d)", k, dense_max_k());
-            return B2_ERANGE;
-        }
-        const bool full_sort = k > dense_select_max_k();  // dense path sorts whole rows: score + two key buffers per column
-        const int64_t rows = std::min<int64_t>(dense_rows_cap(X.n, full_sort), nq);
-        B2_TRY(idx->dense.ensure((size_t)rows * X.n * sizeof(float)));
-        if (full_sort) B2_TRY(idx->sort_keys.ensure(dense_sort_ws_bytes(rows, X.n)));
-        B2_TRY(launch_dense_topk(X, q_dev, q_dtype, nq, nullptr, nq, metric, k, id_map, id_offset, idx->dense.as<float>(), rows,
-                                 full_sort ? idx->sort_keys.as<uint64_t>() : nullptr, out_sc, out_id, st));
-        g_stats[ST_FALLBACK] += nq;
-        return B2_OK;
-    }
-    int64_t n_deferred = 0;
-    for (const FilterChunk& c : p.chunks) {
-        B2_TRY(run_filter(idx, p, c, metric, st));
-        int64_t n_sel = 0;
-        B2_TRY(certify(idx, p, c, metric, id_map, id_offset, out_sc, out_id, nullptr, /*fallback=*/!p.two_level, &n_sel, st));
-        if (p.two_level && n_sel > 0) {
-            B2_TRY(idx->defer.ensure((size_t)nq * sizeof(int64_t)));
-            defer_append_kernel<<<(unsigned)ceil_div(n_sel, 256), 256, 0, st>>>(idx->sel.as<int32_t>() + 1, n_sel, c.q0,
-                                                                               idx->defer.as<int64_t>() + n_deferred);
-            B2_LAUNCH_CHECK();
-            n_deferred += n_sel;
-        }
-    }
-    if (n_deferred > 0) {
-        // second level: the deferred queries against the exact-operand (tf32) filter of the same store
-        const size_t qrow = (size_t)X.d * esize(q_dtype);
-        B2_TRY(idx->q_sub.ensure((size_t)n_deferred * qrow));
-        B2_TRY(idx->sub_sc.ensure((size_t)n_deferred * k * sizeof(float)));
-        B2_TRY(idx->sub_id.ensure((size_t)n_deferred * k * sizeof(int64_t)));
-        B2_TRY(idx->scalar.ensure(64));
-        int* err = reinterpret_cast<int*>(idx->scalar.as<char>() + 16);
-        B2_TRY(launch_gather_rows(q_dev, q_dtype, X.d, idx->defer.as<int64_t>(), n_deferred, nq, idx->q_sub.p, err, st));
-        MatView X2 = X_in;
-        X2.filt16 = nullptr;
-        B2_TRY(search_core(idx, X2, metric, idx->q_sub.p, q_dtype, n_deferred, k, id_map, id_offset, idx->sub_sc.as<float>(),
-                           idx->sub_id.as<int64_t>(), st, /*level=*/1));
-        scatter_rows_kernel<<<(unsigned)ceil_div(n_deferred * k, 256), 256, 0, st>>>(idx->defer.as<int64_t>(), n_deferred, k, idx->sub_sc.as<float>(),
-                                                                                    idx->sub_id.as<int64_t>(), out_sc, out_id);
-        B2_LAUNCH_CHECK();
-        g_stats[ST_SECOND_LEVEL] += n_deferred;
-    }
-    return B2_OK;
 }
 
 int gather_rows_checked(const void* x, int dtype, int d, const int64_t* ids, int64_t m, int64_t n, void* out, DevBuf& scalar,
@@ -493,254 +401,6 @@ static MatView host_view(HostRows& H) {
     return v;
 }
 
-// The filter plan of one chunk (every chunk streams chunk_rows rows, so one plan serves them all). Level 1 (the second level of
-// an fp32 store) streams the fp32 rows; level 0 of an fp32 store streams the bf16 copy when the plan takes two levels.
-static int host_plan(b2_index* idx, HostRows& H, const void* q_dev, int q_dtype, int64_t nq, int k, int level, FilterPlan& p) {
-    MatView Xc = host_view(H);
-    Xc.n = H.chunk_rows;
-    if (level == 0 && H.rows16.p) {
-        Xc.filt16 = H.rows16.dev;  // (the plan only tests it; each chunk's slot replaces it)
-        Xc.filt16_pitch = round_up(H.d, tma_align_elems(B2_BF16));
-    }
-    if (H.dtype == B2_I8 && q_dtype != B2_I8) {
-        Xc.filt_f16 = H.rows.dev;  // (likewise: each chunk's fp16 form replaces it)
-        Xc.filt_f16_pitch = round_up(H.d, tma_align_elems(B2_F16));
-    }
-    return plan_filter(Xc, q_dev, q_dtype, nq, k, false, idx->device, p);
-}
-
-static int ensure_events(std::vector<cudaEvent_t>& ev, size_t count) {
-    while (ev.size() < count) {
-        cudaEvent_t e = nullptr;
-        B2_CUDA(cudaEventCreate(&e));
-        ev.push_back(e);
-    }
-    return B2_OK;
-}
-
-// Filter the query chunk qc of plan p over every corpus chunk of H (copy of chunk c + 1 on the copy stream while chunk c is
-// filtered) and fold the lists into hs.run_* ([qc.nq, cap] and [qc.nq]).
-static int stream_filter_fold(b2_index* idx, HostRows& H, const FilterPlan& p, const FilterChunk& qc, int metric, int cap,
-                              cudaStream_t st) {
-    HostStore& hs = *idx->host;
-    const int d = H.d;
-    const bool via_f16 = p.X.filt_dtype == B2_F16 && H.dtype == B2_I8;  // float queries on an int8 store
-    const int src_dtype = p.two_level ? B2_BF16 : H.dtype;
-    const char* src = reinterpret_cast<const char*>(p.two_level ? H.rows16.p : H.rows.p);
-    const size_t src_row = (size_t)d * esize(src_dtype);
-    const size_t slot_pitch = via_f16 ? src_row : (size_t)p.X.filt_pitch * esize(src_dtype);
-    const int64_t R = H.chunk_rows;
-    for (int s = 0; s < HostStore::SLOTS; ++s) {
-        B2_TRY(hs.slot[s].ensure((size_t)R * slot_pitch));
-        if (via_f16) B2_TRY(hs.slot16[s].ensure((size_t)R * p.X.filt_pitch * 2));
-    }
-    // the queries in the filter's form, once for every corpus chunk
-    FilterPlan pc = p;
-    FilterChunk c = qc;
-    c.q0 = 0;
-    const void* qsrc = reinterpret_cast<const char*>(p.q) + (size_t)qc.q0 * d * esize(p.q_dtype);
-    pc.q = qsrc;
-    if (!p.q_in_place) {
-        B2_TRY(idx->q_filt.ensure((size_t)qc.nq * p.q_pitch * esize(p.X.filt_dtype)));
-        B2_TRY(launch_prep_queries(qsrc, p.q_dtype, qc.nq, d, idx->q_filt.p, p.X.filt_dtype, p.q_pitch, st));
-        pc.q = idx->q_filt.p;
-        pc.q_in_place = true;
-    }
-    B2_TRY(hs.run_score.ensure((size_t)qc.nq * cap * sizeof(float)));
-    B2_TRY(hs.run_id.ensure((size_t)qc.nq * cap * sizeof(int32_t)));
-    B2_TRY(hs.run_thr.ensure((size_t)qc.nq * sizeof(float)));
-    B2_CUDA(cudaMemsetAsync(hs.run_id.p, 0xFF, (size_t)qc.nq * cap * sizeof(int32_t), st));
-    B2_TRY(launch_fill_f32(hs.run_thr.as<float>(), qc.nq, -INFINITY, st));
-    const int nc = H.n_chunks;
-    B2_TRY(ensure_events(hs.ev, (size_t)4 * nc));
-    auto issue_copy = [&](int ch) -> int {
-        const int s = ch % HostStore::SLOTS;
-        const int64_t base = std::min<int64_t>((int64_t)ch * R, H.n - R);
-        B2_CUDA(cudaStreamWaitEvent(hs.copy, hs.freed[s], 0));  // the slot's previous chunk has been filtered
-        B2_CUDA(cudaEventRecord(hs.ev[4 * ch], hs.copy));
-        B2_CUDA(cudaMemcpy2DAsync(hs.slot[s].p, slot_pitch, src + (size_t)base * src_row, src_row, src_row, (size_t)R,
-                                  cudaMemcpyHostToDevice, hs.copy));
-        B2_CUDA(cudaEventRecord(hs.ev[4 * ch + 1], hs.copy));
-        B2_CUDA(cudaEventRecord(hs.copied[s], hs.copy));
-        g_stats[ST_STREAM_BYTES] += R * (int64_t)src_row;
-        return B2_OK;
-    };
-    B2_CUDA(cudaEventRecord(hs.span0, st));
-    B2_TRY(issue_copy(0));
-    for (int ch = 0; ch < nc; ++ch) {
-        if (ch + 1 < nc) B2_TRY(issue_copy(ch + 1));
-        const int s = ch % HostStore::SLOTS;
-        const int64_t base = std::min<int64_t>((int64_t)ch * R, H.n - R);
-        B2_CUDA(cudaStreamWaitEvent(st, hs.copied[s], 0));
-        pc.X = p.X;
-        if (via_f16) {
-            B2_TRY(launch_convert_pad(hs.slot[s].p, B2_I8, R, d, hs.slot16[s].p, B2_F16, p.X.filt_pitch, st));
-            pc.X.filt = hs.slot16[s].p;
-        } else {
-            pc.X.filt = hs.slot[s].p;
-        }
-        pc.X.store = pc.X.filt;
-        pc.X.norm2 = p.X.norm2 + base;
-        pc.X.norm2_i8 = p.X.norm2_i8 ? p.X.norm2_i8 + base : nullptr;
-        if (p.X.mask) {
-            // the chunk's rows start at a word of the mask, except those of a last chunk that re-streams its predecessor's tail
-            if (base % 32 == 0) {
-                pc.X.mask = p.X.mask + base / 32;
-            } else {
-                const int64_t words = ceil_div(R, 32);
-                B2_TRY(hs.mask_slice.ensure((size_t)words * sizeof(uint32_t)));
-                mask_slice_kernel<<<(unsigned)std::min<int64_t>(ceil_div(words, 256), 1024), 256, 0, st>>>(p.X.mask, base, H.n, words,
-                                                                                                      hs.mask_slice.as<uint32_t>());
-                B2_LAUNCH_CHECK();
-                pc.X.mask = hs.mask_slice.as<uint32_t>();
-            }
-        }
-        B2_CUDA(cudaEventRecord(hs.ev[4 * ch + 2], st));
-        B2_TRY(run_filter(idx, pc, c, metric, st));
-        B2_CUDA(cudaEventRecord(hs.ev[4 * ch + 3], st));
-        B2_CUDA(cudaEventRecord(hs.freed[s], st));  // the slot may take its next chunk
-        B2_TRY(launch_fold_lists(idx->cand_score.as<float>(), idx->cand_id.as<int32_t>(), idx->cand_thr.as<float>(), c.nq,
-                                 2 * c.n_splits, p.kp / 2, base, (int64_t)ch * R - base, cap, hs.run_score.as<float>(),
-                                 hs.run_id.as<int32_t>(), hs.run_thr.as<float>(), st));
-        g_stats[ST_STREAM_CHUNKS]++;
-    }
-    B2_CUDA(cudaEventRecord(hs.span1, st));
-    return B2_OK;
-}
-
-// event times of the last stream_filter_fold (after the search stream was synchronised)
-static void stream_times_add(b2_index* idx, int nc) {
-    HostStore& hs = *idx->host;
-    float ms = 0.f, filt = 0.f;
-    for (int ch = 0; ch < nc; ++ch) {
-        if (cudaEventElapsedTime(&ms, hs.ev[4 * ch], hs.ev[4 * ch + 1]) == cudaSuccess) hs.copy_ms += ms;
-        if (cudaEventElapsedTime(&ms, hs.ev[4 * ch + 2], hs.ev[4 * ch + 3]) == cudaSuccess) filt += ms;
-    }
-    if (cudaEventElapsedTime(&ms, hs.span0, hs.span1) == cudaSuccess) hs.span_ms += ms;
-    hs.filter_ms += filt;
-    idx->last_filter_ms = (idx->last_filter_ms < 0 ? 0.f : idx->last_filter_ms) + filt;
-}
-
-// The streamed search of the rows H (level as in search_core: level 1 is the tf32 second level of an fp32 store, which streams
-// the fp32 rows). Results are those of search_core over the same rows in device memory, bit for bit.
-// mask: MatView::mask over the rows of H (null = every row).
-static int stream_search(b2_index* idx, HostRows& H, int metric, const void* q_dev, int q_dtype, int64_t nq, int k,
-                         const int64_t* id_map, int64_t id_offset, float* out_sc, int64_t* out_id, cudaStream_t st, int level,
-                         const uint32_t* mask = nullptr) {
-    HostStore& hs = *idx->host;
-    if (level == 0) {
-        idx->last_filter_ms = -1.f;
-        hs.copy_ms = hs.span_ms = hs.filter_ms = hs.finalize_ms = 0.f;
-    }
-    if (nq <= 0) return B2_OK;
-    if (level == 0) g_stats[ST_QUERIES] += nq;
-    if (H.n <= 0) {
-        fill_pad_kernel<<<132, 256, 0, st>>>(out_sc, out_id, nq * k, metric == B2_METRIC_L2 ? FLT_MAX : -FLT_MAX);
-        B2_LAUNCH_CHECK();
-        return B2_OK;
-    }
-    MatView Xw = host_view(H);
-    Xw.mask = mask;
-    FilterPlan p;
-    B2_TRY(host_plan(idx, H, q_dev, q_dtype, nq, k, level, p));
-    p.X.mask = mask;
-    const int cap = p.use_filter ? finalize_capacity(p.kp, k) : 0;
-    if (!p.use_filter || cap == 0) {
-        // the dense path over every row, read through the mapped pointer
-        if (k > dense_max_k()) {
-            set_error("k=%d is not supported (max %d)", k, dense_max_k());
-            return B2_ERANGE;
-        }
-        const bool full_sort = k > dense_select_max_k();
-        const int64_t rows = std::min<int64_t>(dense_rows_cap(Xw.n, full_sort), nq);
-        B2_TRY(idx->dense.ensure((size_t)rows * Xw.n * sizeof(float)));
-        if (full_sort) B2_TRY(idx->sort_keys.ensure(dense_sort_ws_bytes(rows, Xw.n)));
-        B2_TRY(launch_dense_topk(Xw, q_dev, q_dtype, nq, nullptr, nq, metric, k, id_map, id_offset, idx->dense.as<float>(), rows,
-                                 full_sort ? idx->sort_keys.as<uint64_t>() : nullptr, out_sc, out_id, st));
-        g_stats[ST_FALLBACK] += nq;
-        return B2_OK;
-    }
-    int64_t n_deferred = 0;
-    for (const FilterChunk& qc : p.chunks) {
-        B2_TRY(stream_filter_fold(idx, H, p, qc, metric, cap, st));
-        const void* qc_ptr = reinterpret_cast<const char*>(q_dev) + (size_t)qc.q0 * H.d * esize(q_dtype);
-        float* osc = out_sc + (size_t)qc.q0 * k;
-        int64_t* oid = out_id + (size_t)qc.q0 * k;
-        B2_TRY(idx->flags.ensure((size_t)qc.nq * sizeof(int32_t)));
-        B2_TRY(idx->sel.ensure((size_t)(qc.nq + 1) * sizeof(int32_t)));
-        B2_TRY(idx->h_flags.ensure(64));
-        int32_t* sel_count = idx->sel.as<int32_t>();
-        int32_t* sel_list = sel_count + 1;
-        B2_CUDA(cudaMemsetAsync(sel_count, 0, sizeof(int32_t), st));
-        B2_CUDA(cudaEventRecord(hs.fin0, st));
-        B2_TRY(launch_finalize(Xw, qc_ptr, q_dtype, qc.nq, metric, k, p.kp, cap, 1, hs.run_score.as<float>(), hs.run_id.as<int32_t>(),
-                               hs.run_thr.as<float>(), p.rel_eps, p.abs_eps, p.q_norm_limit, id_map, id_offset, osc, oid,
-                               idx->flags.as<int32_t>(), sel_list, sel_count, st, nullptr));
-        B2_CUDA(cudaEventRecord(hs.fin1, st));
-        int32_t* h_count = reinterpret_cast<int32_t*>(idx->h_flags.p);
-        B2_CUDA(cudaMemcpyAsync(h_count, sel_count, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-        cudaError_t se = cudaStreamSynchronize(st);
-        if (se != cudaSuccess) {
-            set_error("streamed search failed on the device: %s", cudaGetErrorString(se));
-            return B2_ECUDA;
-        }
-        stream_times_add(idx, H.n_chunks);
-        float ms = 0.f;
-        if (cudaEventElapsedTime(&ms, hs.fin0, hs.fin1) == cudaSuccess) hs.finalize_ms += ms;
-        const int64_t n_sel = *h_count;
-        if (n_sel == 0) continue;
-        if (p.two_level) {
-            B2_TRY(idx->defer.ensure((size_t)nq * sizeof(int64_t)));
-            defer_append_kernel<<<(unsigned)ceil_div(n_sel, 256), 256, 0, st>>>(sel_list, n_sel, qc.q0, idx->defer.as<int64_t>() + n_deferred);
-            B2_LAUNCH_CHECK();
-            n_deferred += n_sel;
-            continue;
-        }
-        // exact dense path for the queries the certificate could not cover
-        g_stats[ST_FALLBACK] += n_sel;
-        const int64_t rows = std::min<int64_t>(dense_rows_cap(Xw.n, false), n_sel);
-        B2_TRY(idx->dense.ensure((size_t)rows * Xw.n * sizeof(float)));
-        B2_TRY(launch_dense_topk(Xw, qc_ptr, q_dtype, qc.nq, sel_list, n_sel, metric, k, id_map, id_offset, idx->dense.as<float>(), rows,
-                                 nullptr, osc, oid, st));
-    }
-    if (n_deferred > 0) {
-        // second level: the deferred queries against the tf32 filter over the streamed fp32 rows
-        const size_t qrow = (size_t)H.d * esize(q_dtype);
-        B2_TRY(idx->q_sub.ensure((size_t)n_deferred * qrow));
-        B2_TRY(idx->sub_sc.ensure((size_t)n_deferred * k * sizeof(float)));
-        B2_TRY(idx->sub_id.ensure((size_t)n_deferred * k * sizeof(int64_t)));
-        B2_TRY(idx->scalar.ensure(64));
-        int* err = reinterpret_cast<int*>(idx->scalar.as<char>() + 16);
-        B2_TRY(launch_gather_rows(q_dev, q_dtype, H.d, idx->defer.as<int64_t>(), n_deferred, nq, idx->q_sub.p, err, st));
-        B2_TRY(stream_search(idx, H, metric, idx->q_sub.p, q_dtype, n_deferred, k, id_map, id_offset, idx->sub_sc.as<float>(),
-                             idx->sub_id.as<int64_t>(), st, /*level=*/1, mask));
-        scatter_rows_kernel<<<(unsigned)ceil_div(n_deferred * k, 256), 256, 0, st>>>(idx->defer.as<int64_t>(), n_deferred, k,
-                                                                                    idx->sub_sc.as<float>(), idx->sub_id.as<int64_t>(),
-                                                                                    out_sc, out_id);
-        B2_LAUNCH_CHECK();
-        g_stats[ST_SECOND_LEVEL] += n_deferred;
-    }
-    return B2_OK;
-}
-
-// A search of a host-resident index: the whole index, or an ids subset (ids_host and / or ids_dev; ids_dev is what the results
-// map through). A subset whose rows fit in the ring is gathered from host memory into a device view and searched as on a
-// device-resident index; a larger one is gathered on the host, by threads, into pinned staging and streamed.
-static int gather_host_subset(b2_index* idx, const int64_t* ids_host, const int64_t* ids_dev, int64_t n_ids, cudaStream_t st);
-
-static int host_search(b2_index* idx, const void* q_dev, int q_dtype, int64_t nq, int k, const int64_t* ids_host, const int64_t* ids_dev,
-                       int64_t n_ids, int64_t id_offset, float* out_sc, int64_t* out_id, cudaStream_t st) {
-    HostStore& hs = *idx->host;
-    if (!ids_dev) return stream_search(idx, hs.main, idx->metric, q_dev, q_dtype, nq, k, nullptr, id_offset, out_sc, out_id, st, 0);
-    if ((size_t)n_ids * ring_row_bytes(idx->d, idx->dtype) <= hs.ring_bytes) {
-        MatView sub;
-        B2_TRY(build_subset(idx, ids_dev, n_ids, q_dtype, sub, st));
-        return search_core(idx, sub, idx->metric, q_dev, q_dtype, nq, k, ids_dev, 0, out_sc, out_id, st);
-    }
-    B2_TRY(gather_host_subset(idx, ids_host, ids_dev, n_ids, st));
-    return stream_search(idx, *hs.sub, idx->metric, q_dev, q_dtype, nq, k, ids_dev, 0, out_sc, out_id, st, 0);
-}
-
 // the rows x[ids] of a host-resident index gathered on the host, by threads, into hs.sub (pinned), with their norms and plan
 static int gather_host_subset(b2_index* idx, const int64_t* ids_host, const int64_t* ids_dev, int64_t n_ids, cudaStream_t st) {
     HostStore& hs = *idx->host;
@@ -768,6 +428,321 @@ static int gather_host_subset(b2_index* idx, const int64_t* ids_host, const int6
     return host_rows_init(S, n_ids, idx->d, idx->dtype, hs.ring_bytes, st);
 }
 
+// The rows a search of idx reads: the whole index, or the ids subset (ids_dev on the device, what the results map through;
+// ids_host the same ids on the host, or null). A subset of a device-resident index, or of a host-resident one whose rows fit
+// in the ring, is gathered into a device view and searched as a device-resident index is; a larger subset of a host-resident
+// index is gathered on the host, by threads, into pinned staging and streamed.
+static int select_rows(b2_index* idx, const int64_t* ids_host, const int64_t* ids_dev, int64_t n_ids, int q_dtype, cudaStream_t st,
+                       SearchRows* rows) {
+    *rows = SearchRows();
+    HostStore* hs = idx->host.get();
+    if (ids_dev && (!hs || (size_t)n_ids * ring_row_bytes(idx->d, idx->dtype) <= hs->ring_bytes))
+        return build_subset(idx, ids_dev, n_ids, q_dtype, rows->X, st);
+    if (!hs) {
+        rows->X = idx->view;
+        return B2_OK;
+    }
+    if (ids_dev) B2_TRY(gather_host_subset(idx, ids_host, ids_dev, n_ids, st));
+    rows->H = ids_dev ? hs->sub.get() : &hs->main;
+    rows->X = host_view(*rows->H);
+    return B2_OK;
+}
+
+// The filter plan of a search of R. For streamed rows it is the plan of one chunk (every chunk streams chunk_rows rows, so one
+// plan serves them all): level 1 (the second level of an fp32 store) streams the fp32 rows; level 0 of an fp32 store streams the
+// bf16 copy when the plan takes two levels.
+static int plan_rows(b2_index* idx, const SearchRows& R, const void* q_dev, int q_dtype, int64_t nq, int k, bool top1, int level,
+                     FilterPlan& p) {
+    if (!R.H) return plan_filter(R.X, q_dev, q_dtype, nq, k, top1, idx->device, p);
+    const HostRows& H = *R.H;
+    MatView Xc = R.X;
+    Xc.n = H.chunk_rows;
+    if (level == 0 && H.rows16.p) {
+        Xc.filt16 = H.rows16.dev;  // (the plan only tests it; each chunk's slot replaces it)
+        Xc.filt16_pitch = round_up(H.d, tma_align_elems(B2_BF16));
+    }
+    if (H.dtype == B2_I8 && q_dtype != B2_I8) {
+        Xc.filt_f16 = H.rows.dev;  // (likewise: each chunk's fp16 form replaces it)
+        Xc.filt_f16_pitch = round_up(H.d, tma_align_elems(B2_F16));
+    }
+    return plan_filter(Xc, q_dev, q_dtype, nq, k, top1, idx->device, p);
+}
+
+static int ensure_events(std::vector<cudaEvent_t>& ev, size_t count) {
+    while (ev.size() < count) {
+        cudaEvent_t e = nullptr;
+        B2_CUDA(cudaEventCreate(&e));
+        ev.push_back(e);
+    }
+    return B2_OK;
+}
+
+// Streams the rows of H through the ring of device slots; the copy of chunk ch + 1 (on the copy stream) is issued before chunk
+// ch is processed. Xc describes every chunk (Xc.n = H.chunk_rows; norms and mask those of all of H), and Xc.filt_dtype names the
+// filter operand: the rows, their bf16 copy (the first level of an fp32 store) or, for float queries on an int8 store, their
+// fp16 form, converted in the slot when `convert`. Chunk ch reaches on_slot(X, pitch, base, own_lo) as the view X of its slot:
+// the rows [base, base + X.n) of H, exact in X.store at `pitch` elements per row, of which the first own_lo belong to the previous
+// chunk (only the last chunk re-streams its predecessor's tail). The slot is released once on_slot's work is queued; then
+// then(base, own_lo) runs.
+template <typename OnSlot, typename Then>
+static int stream_chunks(b2_index* idx, HostRows& H, const MatView& Xc, bool convert, cudaStream_t st, const OnSlot& on_slot,
+                         const Then& then) {
+    HostStore& hs = *idx->host;
+    const int d = H.d;
+    const bool via_f16 = Xc.filt_dtype == B2_F16 && H.dtype == B2_I8;
+    const int src_dtype = via_f16 ? H.dtype : Xc.filt_dtype;
+    const char* src = reinterpret_cast<const char*>(src_dtype == H.dtype ? H.rows.p : H.rows16.p);
+    const size_t src_row = (size_t)d * esize(src_dtype);
+    const int64_t pitch = via_f16 ? d : round_up(d, tma_align_elems(src_dtype));  // elements per slot row
+    const size_t slot_pitch = (size_t)pitch * esize(src_dtype);
+    const int64_t f16_pitch = round_up(d, tma_align_elems(B2_F16));
+    const int64_t R = H.chunk_rows;
+    for (int s = 0; s < HostStore::SLOTS; ++s) {
+        B2_TRY(hs.slot[s].ensure((size_t)R * slot_pitch));
+        if (via_f16) B2_TRY(hs.slot16[s].ensure((size_t)R * f16_pitch * 2));
+    }
+    const int nc = H.n_chunks;
+    B2_TRY(ensure_events(hs.ev, (size_t)4 * nc));
+    auto issue_copy = [&](int ch) -> int {
+        const int s = ch % HostStore::SLOTS;
+        const int64_t base = std::min<int64_t>((int64_t)ch * R, H.n - R);
+        B2_CUDA(cudaStreamWaitEvent(hs.copy, hs.freed[s], 0));  // the slot's previous chunk has been processed
+        B2_CUDA(cudaEventRecord(hs.ev[4 * ch], hs.copy));
+        B2_CUDA(cudaMemcpy2DAsync(hs.slot[s].p, slot_pitch, src + (size_t)base * src_row, src_row, src_row, (size_t)R,
+                                  cudaMemcpyHostToDevice, hs.copy));
+        B2_CUDA(cudaEventRecord(hs.ev[4 * ch + 1], hs.copy));
+        B2_CUDA(cudaEventRecord(hs.copied[s], hs.copy));
+        g_stats[ST_STREAM_BYTES] += R * (int64_t)src_row;
+        return B2_OK;
+    };
+    B2_CUDA(cudaEventRecord(hs.span0, st));
+    B2_TRY(issue_copy(0));
+    for (int ch = 0; ch < nc; ++ch) {
+        if (ch + 1 < nc) B2_TRY(issue_copy(ch + 1));
+        const int s = ch % HostStore::SLOTS;
+        const int64_t base = std::min<int64_t>((int64_t)ch * R, H.n - R);
+        B2_CUDA(cudaStreamWaitEvent(st, hs.copied[s], 0));
+        MatView X = Xc;
+        X.store = X.filt = hs.slot[s].p;
+        X.filt_pitch = pitch;
+        if (via_f16) {
+            if (convert) B2_TRY(launch_convert_pad(hs.slot[s].p, B2_I8, R, d, hs.slot16[s].p, B2_F16, f16_pitch, st));
+            X.filt = hs.slot16[s].p;
+            X.filt_pitch = f16_pitch;
+        }
+        X.norm2 = Xc.norm2 + base;
+        X.norm2_i8 = Xc.norm2_i8 ? Xc.norm2_i8 + base : nullptr;
+        if (Xc.mask) {
+            // the chunk's rows start at a word of the mask, except those of a last chunk that re-streams its predecessor's tail
+            if (base % 32 == 0) {
+                X.mask = Xc.mask + base / 32;
+            } else {
+                const int64_t words = ceil_div(R, 32);
+                B2_TRY(hs.mask_slice.ensure((size_t)words * sizeof(uint32_t)));
+                mask_slice_kernel<<<(unsigned)std::min<int64_t>(ceil_div(words, 256), 1024), 256, 0, st>>>(Xc.mask, base, H.n, words,
+                                                                                                      hs.mask_slice.as<uint32_t>());
+                B2_LAUNCH_CHECK();
+                X.mask = hs.mask_slice.as<uint32_t>();
+            }
+        }
+        B2_CUDA(cudaEventRecord(hs.ev[4 * ch + 2], st));
+        B2_TRY(on_slot(X, pitch, base, (int64_t)ch * R - base));
+        B2_CUDA(cudaEventRecord(hs.ev[4 * ch + 3], st));
+        B2_CUDA(cudaEventRecord(hs.freed[s], st));  // the slot may take its next chunk
+        B2_TRY(then(base, (int64_t)ch * R - base));
+        g_stats[ST_STREAM_CHUNKS]++;
+    }
+    B2_CUDA(cudaEventRecord(hs.span1, st));
+    return B2_OK;
+}
+
+// Filter the query chunk qc of plan p over every corpus chunk of H and fold the lists into hs.run_* ([qc.nq, cap] and [qc.nq]).
+static int stream_filter_fold(b2_index* idx, HostRows& H, const FilterPlan& p, const FilterChunk& qc, int metric, int cap,
+                              cudaStream_t st) {
+    HostStore& hs = *idx->host;
+    // the queries in the filter's form, once for every corpus chunk
+    FilterPlan pc = p;
+    FilterChunk c = qc;
+    c.q0 = 0;
+    const void* qsrc = reinterpret_cast<const char*>(p.q) + (size_t)qc.q0 * H.d * esize(p.q_dtype);
+    pc.q = qsrc;
+    if (!p.q_in_place) {
+        B2_TRY(idx->q_filt.ensure((size_t)qc.nq * p.q_pitch * esize(p.X.filt_dtype)));
+        B2_TRY(launch_prep_queries(qsrc, p.q_dtype, qc.nq, H.d, idx->q_filt.p, p.X.filt_dtype, p.q_pitch, st));
+        pc.q = idx->q_filt.p;
+        pc.q_in_place = true;
+    }
+    B2_TRY(hs.run_score.ensure((size_t)qc.nq * cap * sizeof(float)));
+    B2_TRY(hs.run_id.ensure((size_t)qc.nq * cap * sizeof(int32_t)));
+    B2_TRY(hs.run_thr.ensure((size_t)qc.nq * sizeof(float)));
+    B2_CUDA(cudaMemsetAsync(hs.run_id.p, 0xFF, (size_t)qc.nq * cap * sizeof(int32_t), st));
+    B2_TRY(launch_fill_f32(hs.run_thr.as<float>(), qc.nq, -INFINITY, st));
+    return stream_chunks(
+        idx, H, p.X, /*convert=*/true, st,
+        [&](const MatView& X, int64_t, int64_t, int64_t) {
+            pc.X = X;
+            return run_filter(idx, pc, c, metric, st);
+        },
+        [&](int64_t base, int64_t own_lo) {
+            const CandLists L = filter_lists(idx, pc, c);
+            return launch_fold_lists(L.score, L.id, L.thr, c.nq, L.n_lists, L.list_len, base, own_lo, cap, hs.run_score.as<float>(),
+                                     hs.run_id.as<int32_t>(), hs.run_thr.as<float>(), st);
+        });
+}
+
+// event times of the last stream_filter_fold and the finalize after it (after the search stream was synchronised)
+static void stream_times_add(b2_index* idx, int nc) {
+    HostStore& hs = *idx->host;
+    float ms = 0.f, filt = 0.f;
+    for (int ch = 0; ch < nc; ++ch) {
+        if (cudaEventElapsedTime(&ms, hs.ev[4 * ch], hs.ev[4 * ch + 1]) == cudaSuccess) hs.copy_ms += ms;
+        if (cudaEventElapsedTime(&ms, hs.ev[4 * ch + 2], hs.ev[4 * ch + 3]) == cudaSuccess) filt += ms;
+    }
+    if (cudaEventElapsedTime(&ms, hs.span0, hs.span1) == cudaSuccess) hs.span_ms += ms;
+    if (cudaEventElapsedTime(&ms, hs.fin0, hs.fin1) == cudaSuccess) hs.finalize_ms += ms;
+    hs.filter_ms += filt;
+    idx->last_filter_ms = (idx->last_filter_ms < 0 ? 0.f : idx->last_filter_ms) + filt;
+}
+
+// The candidate lists of query chunk c of a search of R: the filter run over a device view, or over every streamed chunk of
+// R.H with the lists folded into one of `cap` entries.
+static int chunk_lists(b2_index* idx, const SearchRows& R, const FilterPlan& p, const FilterChunk& c, int metric, int cap,
+                       CandLists* L, cudaStream_t st) {
+    if (!R.H) {
+        B2_TRY(run_filter(idx, p, c, metric, st));
+        *L = filter_lists(idx, p, c);
+        return B2_OK;
+    }
+    B2_TRY(stream_filter_fold(idx, *R.H, p, c, metric, cap, st));
+    HostStore& hs = *idx->host;
+    *L = {hs.run_score.as<float>(), hs.run_id.as<int32_t>(), hs.run_thr.as<float>(), cap, 1};
+    return B2_OK;
+}
+
+// Finalize/certify the lists L of chunk c over the rows R (hint: a lower bound the k-th score is known to reach, or null), read
+// the one counter back and add the filter's event time to idx->last_filter_ms (for streamed rows: every chunk's, with the
+// copy, span and finalize times in the stream times). The queries the certificate leaves open are compacted into
+// idx->sel[1 .. 1 + *n_open]; with `fallback` the exact dense path answers them here.
+static int certify(b2_index* idx, const FilterPlan& p, const FilterChunk& c, const SearchRows& R, const CandLists& L, int metric,
+                   const int64_t* id_map, int64_t id_offset, float* out_sc, int64_t* out_id, const float* hint, bool fallback,
+                   int64_t* n_open, cudaStream_t st) {
+    const MatView& X = R.X;
+    const void* qc = reinterpret_cast<const char*>(p.q) + (size_t)c.q0 * X.d * esize(p.q_dtype);
+    float* osc = out_sc + (size_t)c.q0 * p.k;
+    int64_t* oid = out_id + (size_t)c.q0 * p.k;
+    B2_TRY(idx->flags.ensure((size_t)c.nq * sizeof(int32_t)));
+    B2_TRY(idx->sel.ensure((size_t)(c.nq + 1) * sizeof(int32_t)));  // [0] = counter, [1..] = uncertified queries
+    B2_TRY(idx->h_flags.ensure(64));
+    int32_t* sel_count = idx->sel.as<int32_t>();
+    int32_t* sel_list = sel_count + 1;
+    B2_CUDA(cudaMemsetAsync(sel_count, 0, sizeof(int32_t), st));
+    if (R.H) B2_CUDA(cudaEventRecord(idx->host->fin0, st));
+    B2_TRY(launch_finalize(X, qc, p.q_dtype, c.nq, metric, p.k, p.kp, L.list_len, L.n_lists, L.score, L.id, L.thr, p.rel_eps,
+                           p.abs_eps, p.q_norm_limit, id_map, id_offset, osc, oid, idx->flags.as<int32_t>(), sel_list, sel_count, st,
+                           hint));
+    if (R.H) B2_CUDA(cudaEventRecord(idx->host->fin1, st));
+    // the certificate outcome comes back as ONE counter (the failed queries are compacted on the device)
+    int32_t* h_count = reinterpret_cast<int32_t*>(idx->h_flags.p);
+    B2_CUDA(cudaMemcpyAsync(h_count, sel_count, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    cudaError_t se = cudaStreamSynchronize(st);
+    if (se != cudaSuccess) {
+        set_error("search pipeline failed on the device: %s", cudaGetErrorString(se));
+        return B2_ECUDA;
+    }
+    float ms = -1.f;
+    if (R.H)
+        stream_times_add(idx, R.H->n_chunks);
+    else if (cudaEventElapsedTime(&ms, idx->ev0, idx->ev1) == cudaSuccess)
+        idx->last_filter_ms = (idx->last_filter_ms < 0 ? 0.f : idx->last_filter_ms) + ms;
+    const int64_t n_sel = *h_count;
+    *n_open = n_sel;
+    if (!fallback || n_sel == 0) return B2_OK;
+    // exact fallback for the queries the certificate could not cover
+    if (p.k > dense_max_k()) {
+        set_error("internal: fallback with k=%d", p.k);
+        return B2_ERANGE;
+    }
+    g_stats[ST_FALLBACK] += n_sel;
+    const int64_t rows = std::min<int64_t>(dense_rows_cap(X.n, false), n_sel);
+    B2_TRY(idx->dense.ensure((size_t)rows * X.n * sizeof(float)));
+    return launch_dense_topk(X, qc, p.q_dtype, c.nq, sel_list, n_sel, metric, p.k, id_map, id_offset, idx->dense.as<float>(), rows,
+                             nullptr, osc, oid, st);
+}
+
+// level 0: the caller's search. On a two-level plan the queries whose first-level certificate fails are deferred, gathered and
+// answered by a level-1 call (tf32 filter on the same store, then the dense path for what still fails) and scattered back.
+// Streamed rows give the results of the same rows in device memory, bit for bit.
+int search_core(b2_index* idx, const SearchRows& R, int metric, const void* q_dev, int q_dtype, int64_t nq, int k,
+                const int64_t* id_map, int64_t id_offset, float* out_sc, int64_t* out_id, cudaStream_t st, int level) {
+    const MatView& X = R.X;
+    if (level == 0) {
+        idx->last_filter_ms = -1.f;
+        if (R.H) {
+            HostStore& hs = *idx->host;
+            hs.copy_ms = hs.span_ms = hs.filter_ms = hs.finalize_ms = 0.f;
+        }
+    }
+    if (nq <= 0) return B2_OK;
+    if (level == 0) g_stats[ST_QUERIES] += nq;
+    if (X.n <= 0) {
+        fill_pad_kernel<<<132, 256, 0, st>>>(out_sc, out_id, nq * k, metric == B2_METRIC_L2 ? FLT_MAX : -FLT_MAX);
+        B2_LAUNCH_CHECK();
+        return B2_OK;
+    }
+    FilterPlan p;
+    B2_TRY(plan_rows(idx, R, q_dev, q_dtype, nq, k, false, level, p));
+    // streamed rows fold their lists into one of `cap` entries, which finalize has to be able to hold
+    const int cap = R.H && p.use_filter ? finalize_capacity(p.kp, k) : 0;
+    if (!p.use_filter || (R.H && cap == 0)) {
+        // the dense path over every row (streamed rows: read through the mapped pointer)
+        if (k > dense_max_k()) {
+            set_error("k=%d is not supported (max %d)", k, dense_max_k());
+            return B2_ERANGE;
+        }
+        const bool full_sort = k > dense_select_max_k();  // dense path sorts whole rows: score + two key buffers per column
+        const int64_t rows = std::min<int64_t>(dense_rows_cap(X.n, full_sort), nq);
+        B2_TRY(idx->dense.ensure((size_t)rows * X.n * sizeof(float)));
+        if (full_sort) B2_TRY(idx->sort_keys.ensure(dense_sort_ws_bytes(rows, X.n)));
+        B2_TRY(launch_dense_topk(X, q_dev, q_dtype, nq, nullptr, nq, metric, k, id_map, id_offset, idx->dense.as<float>(), rows,
+                                 full_sort ? idx->sort_keys.as<uint64_t>() : nullptr, out_sc, out_id, st));
+        g_stats[ST_FALLBACK] += nq;
+        return B2_OK;
+    }
+    int64_t n_deferred = 0;
+    for (const FilterChunk& c : p.chunks) {
+        CandLists L;
+        B2_TRY(chunk_lists(idx, R, p, c, metric, cap, &L, st));
+        int64_t n_sel = 0;
+        B2_TRY(certify(idx, p, c, R, L, metric, id_map, id_offset, out_sc, out_id, nullptr, /*fallback=*/!p.two_level, &n_sel, st));
+        if (p.two_level && n_sel > 0) {
+            B2_TRY(idx->defer.ensure((size_t)nq * sizeof(int64_t)));
+            defer_append_kernel<<<(unsigned)ceil_div(n_sel, 256), 256, 0, st>>>(idx->sel.as<int32_t>() + 1, n_sel, c.q0,
+                                                                               idx->defer.as<int64_t>() + n_deferred);
+            B2_LAUNCH_CHECK();
+            n_deferred += n_sel;
+        }
+    }
+    if (n_deferred > 0) {
+        // second level: the deferred queries against the exact-operand (tf32) filter of the same store
+        const size_t qrow = (size_t)X.d * esize(q_dtype);
+        B2_TRY(idx->q_sub.ensure((size_t)n_deferred * qrow));
+        B2_TRY(idx->sub_sc.ensure((size_t)n_deferred * k * sizeof(float)));
+        B2_TRY(idx->sub_id.ensure((size_t)n_deferred * k * sizeof(int64_t)));
+        B2_TRY(idx->scalar.ensure(64));
+        int* err = reinterpret_cast<int*>(idx->scalar.as<char>() + 16);
+        B2_TRY(launch_gather_rows(q_dev, q_dtype, X.d, idx->defer.as<int64_t>(), n_deferred, nq, idx->q_sub.p, err, st));
+        SearchRows R2 = R;
+        R2.X.filt16 = nullptr;
+        B2_TRY(search_core(idx, R2, metric, idx->q_sub.p, q_dtype, n_deferred, k, id_map, id_offset, idx->sub_sc.as<float>(),
+                           idx->sub_id.as<int64_t>(), st, /*level=*/1));
+        scatter_rows_kernel<<<(unsigned)ceil_div(n_deferred * k, 256), 256, 0, st>>>(idx->defer.as<int64_t>(), n_deferred, k, idx->sub_sc.as<float>(),
+                                                                                    idx->sub_id.as<int64_t>(), out_sc, out_id);
+        B2_LAUNCH_CHECK();
+        g_stats[ST_SECOND_LEVEL] += n_deferred;
+    }
+    return B2_OK;
+}
+
 // ---- range search (range.cu) ----------------------------------------------------------------------------------------------
 // The filter operand of a device-resident view: float queries on an int8 store use its fp16 copy (exact). An fp32 store filters
 // with tf32 on its own rows (its bf16 first-level copy is a knn optimisation; a range search would only admit more candidates).
@@ -781,84 +756,25 @@ static MatView range_filter_view(const MatView& X, int q_dtype) {
     return v;
 }
 
-static int range_device(b2_index* idx, RangeWork& W, const MatView& X, const void* q_dev, int q_dtype, int64_t nq, float radius,
-                        cudaStream_t st) {
-    B2_TRY(range_begin(idx, W, X, idx->metric, q_dev, q_dtype, nq, radius, st));
-    return range_pass(idx, W, range_filter_view(X, q_dtype), X.d, 0, 0, st);
-}
-
-// The range search of streamed rows H: every chunk is filtered and verified while its slot holds it (the copy of the next chunk
-// runs meanwhile), so verification reads device memory only; the last chunk skips the rows its predecessor covered. An int8
-// store with float queries converts each chunk to fp16 for the filter and verifies against the int8 rows.
-static int range_stream(b2_index* idx, RangeWork& W, HostRows& H, const void* q_dev, int q_dtype, int64_t nq, float radius,
-                        cudaStream_t st) {
-    HostStore& hs = *idx->host;
-    MatView Xc = host_view(H);
-    Xc.n = H.chunk_rows;
+// The range search of R: one pass over a device view, or one pass per streamed chunk, filtered and verified while its slot holds
+// it (the copy of the next chunk runs meanwhile), so verification reads device memory only; the last chunk skips the rows its
+// predecessor covered. An int8 store with float queries filters the fp16 form of each chunk and verifies against the int8 rows.
+static int range_rows(b2_index* idx, RangeWork& W, const SearchRows& R, const void* q_dev, int q_dtype, int64_t nq, float radius,
+                      cudaStream_t st) {
+    if (!R.H) {
+        B2_TRY(range_begin(idx, W, R.X, idx->metric, q_dev, q_dtype, nq, radius, st));
+        return range_pass(idx, W, range_filter_view(R.X, q_dtype), R.X.d, 0, 0, st);
+    }
+    MatView Xc = R.X;
+    Xc.n = R.H->chunk_rows;
     B2_TRY(range_begin(idx, W, Xc, idx->metric, q_dev, q_dtype, nq, radius, st));
-    if (nq <= 0 || H.n <= 0) return B2_OK;
-    const int d = H.d;
-    const bool via_f16 = H.dtype == B2_I8 && q_dtype != B2_I8;
-    const size_t src_row = (size_t)d * esize(H.dtype);
-    const int64_t pitch = via_f16 ? d : Xc.filt_pitch;  // elements per slot row
-    const size_t slot_pitch = (size_t)pitch * esize(H.dtype);
-    const int64_t f16_pitch = round_up(d, tma_align_elems(B2_F16));
-    const int64_t R = H.chunk_rows;
-    for (int s = 0; s < HostStore::SLOTS; ++s) {
-        B2_TRY(hs.slot[s].ensure((size_t)R * slot_pitch));
-        if (via_f16) B2_TRY(hs.slot16[s].ensure((size_t)R * f16_pitch * 2));
-    }
-    const char* src = reinterpret_cast<const char*>(H.rows.p);
-    auto issue_copy = [&](int ch) -> int {
-        const int s = ch % HostStore::SLOTS;
-        const int64_t base = std::min<int64_t>((int64_t)ch * R, H.n - R);
-        B2_CUDA(cudaStreamWaitEvent(hs.copy, hs.freed[s], 0));  // the slot's previous chunk has been verified
-        B2_CUDA(cudaMemcpy2DAsync(hs.slot[s].p, slot_pitch, src + (size_t)base * src_row, src_row, src_row, (size_t)R,
-                                  cudaMemcpyHostToDevice, hs.copy));
-        B2_CUDA(cudaEventRecord(hs.copied[s], hs.copy));
-        g_stats[ST_STREAM_BYTES] += R * (int64_t)src_row;
-        return B2_OK;
-    };
-    const int nc = H.n_chunks;
-    B2_TRY(issue_copy(0));
-    for (int ch = 0; ch < nc; ++ch) {
-        if (ch + 1 < nc) B2_TRY(issue_copy(ch + 1));
-        const int s = ch % HostStore::SLOTS;
-        const int64_t base = std::min<int64_t>((int64_t)ch * R, H.n - R);
-        B2_CUDA(cudaStreamWaitEvent(st, hs.copied[s], 0));
-        MatView Xs = Xc;
-        Xs.store = hs.slot[s].p;
-        Xs.filt = hs.slot[s].p;
-        Xs.filt_pitch = pitch;
-        Xs.filt_dtype = H.dtype;
-        if (via_f16) {
-            if (W.use_filter) B2_TRY(launch_convert_pad(hs.slot[s].p, B2_I8, R, d, hs.slot16[s].p, B2_F16, f16_pitch, st));
-            Xs.filt = hs.slot16[s].p;
-            Xs.filt_pitch = f16_pitch;
-            Xs.filt_dtype = B2_F16;
-        }
-        Xs.norm2 = Xc.norm2 + base;
-        Xs.norm2_i8 = Xc.norm2_i8 ? Xc.norm2_i8 + base : nullptr;
-        B2_TRY(range_pass(idx, W, Xs, pitch, base, (int64_t)ch * R - base, st));  // synchronises: the slot is free afterwards
-        B2_CUDA(cudaEventRecord(hs.freed[s], st));
-        g_stats[ST_STREAM_CHUNKS]++;
-    }
-    return B2_OK;
-}
-
-// A range search of a host-resident index: the whole index streamed, or an ids subset (gathered into a device view when its rows
-// fit in the ring, else gathered on the host and streamed), as host_search does. *id_map: what the hit positions map through.
-static int host_range(b2_index* idx, RangeWork& W, const void* q_dev, int q_dtype, int64_t nq, float radius, const int64_t* ids_host,
-                      const int64_t* ids_dev, int64_t n_ids, cudaStream_t st) {
-    HostStore& hs = *idx->host;
-    if (!ids_dev) return range_stream(idx, W, hs.main, q_dev, q_dtype, nq, radius, st);
-    if ((size_t)n_ids * ring_row_bytes(idx->d, idx->dtype) <= hs.ring_bytes) {
-        MatView sub;
-        B2_TRY(build_subset(idx, ids_dev, n_ids, q_dtype, sub, st));
-        return range_device(idx, W, sub, q_dev, q_dtype, nq, radius, st);
-    }
-    B2_TRY(gather_host_subset(idx, ids_host, ids_dev, n_ids, st));
-    return range_stream(idx, W, *hs.sub, q_dev, q_dtype, nq, radius, st);
+    if (nq <= 0 || R.H->n <= 0) return B2_OK;
+    return stream_chunks(
+        idx, *R.H, range_filter_view(Xc, q_dtype), /*convert=*/W.use_filter, st,
+        [&](const MatView& X, int64_t pitch, int64_t base, int64_t own_lo) {
+            return range_pass(idx, W, X, pitch, base, own_lo, st);  // synchronises: the slot is free afterwards
+        },
+        [](int64_t, int64_t) { return B2_OK; });
 }
 
 }  // namespace b2
@@ -1072,6 +988,36 @@ static int check_search_args(b2_index* idx, const void* q, int64_t nq, int32_t q
     return B2_OK;
 }
 
+// The inputs of a call on host buffers, staged on the device: the queries in idx->q_in (then adapted, see adapt_queries) and,
+// unless they list every row in order, the ids in idx->ids_dev (*ids_dev = null: the whole index).
+static int stage_host_call(b2_index* idx, const void* q, int64_t nq, int32_t& q_dtype, const int64_t* ids, int64_t n_ids,
+                           cudaStream_t st, const void** q_dev, const int64_t** ids_dev) {
+    const size_t qbytes = (size_t)nq * idx->d * esize(q_dtype);
+    B2_TRY(idx->q_in.ensure(qbytes));
+    B2_CUDA(cudaMemcpyAsync(idx->q_in.p, q, qbytes, cudaMemcpyHostToDevice, st));
+    *q_dev = idx->q_in.p;
+    B2_TRY(adapt_queries(idx, *q_dev, q_dtype, nq, st));
+    *ids_dev = nullptr;
+    if (!ids) return B2_OK;
+    if (n_ids < 0) { set_error("n_ids < 0"); return B2_EINVAL; }
+    bool identity = n_ids == idx->n;
+    for (int64_t i = 0; identity && i < n_ids; ++i) identity = ids[i] == i;
+    if (identity) return B2_OK;
+    B2_TRY(idx->ids_dev.ensure((size_t)std::max<int64_t>(n_ids, 1) * sizeof(int64_t)));
+    B2_CUDA(cudaMemcpyAsync(idx->ids_dev.p, ids, (size_t)n_ids * sizeof(int64_t), cudaMemcpyHostToDevice, st));
+    *ids_dev = idx->ids_dev.as<int64_t>();
+    return B2_OK;
+}
+
+// the top-k results of a call on host buffers (idx->out_sc / out_id, sized for nq x k) copied back, waited for
+static int download_topk(b2_index* idx, int64_t nq, int k, float* out_scores, int64_t* out_idx, cudaStream_t st) {
+    B2_CUDA(cudaMemcpyAsync(out_scores, idx->out_sc.p, (size_t)nq * k * sizeof(float), cudaMemcpyDeviceToHost, st));
+    B2_CUDA(cudaMemcpyAsync(out_idx, idx->out_id.p, (size_t)nq * k * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    cudaError_t e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) { set_error("search failed on the device: %s", cudaGetErrorString(e)); return B2_ECUDA; }
+    return B2_OK;
+}
+
 int b2_index_search_dev(b2_index* idx, const void* q_dev, int64_t nq, int32_t q_dtype, int32_t k, const int64_t* ids_dev,
                         int64_t n_ids, int64_t id_offset, float* out_scores_dev, int64_t* out_idx_dev, void* stream) {
     B2_TRY(check_search_args(idx, q_dev, nq, q_dtype, k));
@@ -1081,15 +1027,9 @@ int b2_index_search_dev(b2_index* idx, const void* q_dev, int64_t nq, int32_t q_
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     B2_TRY(adapt_queries(idx, q_dev, q_dtype, nq, st));
     if (ids_dev && n_ids < 0) { set_error("n_ids < 0"); return B2_EINVAL; }
-    if (idx->host) {
-        B2_TRY(host_search(idx, q_dev, q_dtype, nq, k, nullptr, ids_dev, n_ids, id_offset, out_scores_dev, out_idx_dev, st));
-    } else if (ids_dev) {
-        MatView sub;
-        B2_TRY(build_subset(idx, ids_dev, n_ids, q_dtype, sub, st));
-        B2_TRY(search_core(idx, sub, idx->metric, q_dev, q_dtype, nq, k, ids_dev, 0, out_scores_dev, out_idx_dev, st));
-    } else {
-        B2_TRY(search_core(idx, idx->view, idx->metric, q_dev, q_dtype, nq, k, nullptr, id_offset, out_scores_dev, out_idx_dev, st));
-    }
+    SearchRows R;
+    B2_TRY(select_rows(idx, nullptr, ids_dev, n_ids, q_dtype, st, &R));
+    B2_TRY(search_core(idx, R, idx->metric, q_dev, q_dtype, nq, k, ids_dev, ids_dev ? 0 : id_offset, out_scores_dev, out_idx_dev, st));
     B2_CUDA(cudaStreamSynchronize(st));
     return B2_OK;
 }
@@ -1101,40 +1041,15 @@ int b2_index_search(b2_index* idx, const void* q, int64_t nq, int32_t q_dtype, i
     if (!out_scores || !out_idx) { set_error("output buffers are NULL"); return B2_EINVAL; }
     DeviceGuard guard(idx->device);
     cudaStream_t st = idx->stream;
-    const size_t qbytes = (size_t)nq * idx->d * esize(q_dtype);
-    B2_TRY(idx->q_in.ensure(qbytes));
     B2_TRY(idx->out_sc.ensure((size_t)nq * k * sizeof(float)));
     B2_TRY(idx->out_id.ensure((size_t)nq * k * sizeof(int64_t)));
-    B2_CUDA(cudaMemcpyAsync(idx->q_in.p, q, qbytes, cudaMemcpyHostToDevice, st));
-    const void* q_dev = idx->q_in.p;
-    B2_TRY(adapt_queries(idx, q_dev, q_dtype, nq, st));
+    const void* q_dev = nullptr;
     const int64_t* ids_dev = nullptr;
-    if (ids) {
-        if (n_ids < 0) { set_error("n_ids < 0"); return B2_EINVAL; }
-        bool identity = n_ids == idx->n;
-        for (int64_t i = 0; identity && i < n_ids; ++i) identity = ids[i] == i;
-        if (!identity) {
-            B2_TRY(idx->ids_dev.ensure((size_t)std::max<int64_t>(n_ids, 1) * sizeof(int64_t)));
-            B2_CUDA(cudaMemcpyAsync(idx->ids_dev.p, ids, (size_t)n_ids * sizeof(int64_t), cudaMemcpyHostToDevice, st));
-            ids_dev = idx->ids_dev.as<int64_t>();
-        }
-    }
-    if (idx->host) {
-        B2_TRY(host_search(idx, q_dev, q_dtype, nq, k, ids_dev ? ids : nullptr, ids_dev, n_ids, 0, idx->out_sc.as<float>(),
-                           idx->out_id.as<int64_t>(), st));
-    } else if (ids_dev) {
-        MatView sub;
-        B2_TRY(build_subset(idx, ids_dev, n_ids, q_dtype, sub, st));
-        B2_TRY(search_core(idx, sub, idx->metric, q_dev, q_dtype, nq, k, ids_dev, 0, idx->out_sc.as<float>(), idx->out_id.as<int64_t>(), st));
-    } else {
-        B2_TRY(search_core(idx, idx->view, idx->metric, q_dev, q_dtype, nq, k, nullptr, 0, idx->out_sc.as<float>(),
-                           idx->out_id.as<int64_t>(), st));
-    }
-    B2_CUDA(cudaMemcpyAsync(out_scores, idx->out_sc.p, (size_t)nq * k * sizeof(float), cudaMemcpyDeviceToHost, st));
-    B2_CUDA(cudaMemcpyAsync(out_idx, idx->out_id.p, (size_t)nq * k * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
-    cudaError_t e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) { set_error("search failed on the device: %s", cudaGetErrorString(e)); return B2_ECUDA; }
-    return B2_OK;
+    B2_TRY(stage_host_call(idx, q, nq, q_dtype, ids, n_ids, st, &q_dev, &ids_dev));
+    SearchRows R;
+    B2_TRY(select_rows(idx, ids, ids_dev, n_ids, q_dtype, st, &R));
+    B2_TRY(search_core(idx, R, idx->metric, q_dev, q_dtype, nq, k, ids_dev, 0, idx->out_sc.as<float>(), idx->out_id.as<int64_t>(), st));
+    return download_topk(idx, nq, k, out_scores, out_idx, st);
 }
 
 // ---- masked search: the rows a bitmap selects, searched in place (no gathered copy of the subset) ----------------------------
@@ -1148,11 +1063,10 @@ static int check_masked_args(b2_index* idx, const void* q, int64_t nq, int32_t q
 // mask_dev: ceil(n / 32) words on the index's device
 static int masked_search(b2_index* idx, const void* q_dev, int q_dtype, int64_t nq, int k, const uint32_t* mask_dev, int64_t id_offset,
                          float* out_sc, int64_t* out_id, cudaStream_t st) {
-    if (idx->host)
-        return stream_search(idx, idx->host->main, idx->metric, q_dev, q_dtype, nq, k, nullptr, id_offset, out_sc, out_id, st, 0, mask_dev);
-    MatView X = idx->view;
-    X.mask = mask_dev;
-    return search_core(idx, X, idx->metric, q_dev, q_dtype, nq, k, nullptr, id_offset, out_sc, out_id, st);
+    SearchRows R;
+    B2_TRY(select_rows(idx, nullptr, nullptr, 0, q_dtype, st, &R));
+    R.X.mask = mask_dev;
+    return search_core(idx, R, idx->metric, q_dev, q_dtype, nq, k, nullptr, id_offset, out_sc, out_id, st);
 }
 
 static int upload_mask(b2_index* idx, const uint32_t* mask, cudaStream_t st) {
@@ -1182,21 +1096,15 @@ int b2_index_search_masked(b2_index* idx, const void* q, int64_t nq, int32_t q_d
     if (!out_scores || !out_idx) { set_error("output buffers are NULL"); return B2_EINVAL; }
     DeviceGuard guard(idx->device);
     cudaStream_t st = idx->stream;
-    const size_t qbytes = (size_t)nq * idx->d * esize(q_dtype);
-    B2_TRY(idx->q_in.ensure(qbytes));
     B2_TRY(idx->out_sc.ensure((size_t)nq * k * sizeof(float)));
     B2_TRY(idx->out_id.ensure((size_t)nq * k * sizeof(int64_t)));
-    B2_CUDA(cudaMemcpyAsync(idx->q_in.p, q, qbytes, cudaMemcpyHostToDevice, st));
+    const void* q_dev = nullptr;
+    const int64_t* no_ids = nullptr;
+    B2_TRY(stage_host_call(idx, q, nq, q_dtype, nullptr, 0, st, &q_dev, &no_ids));
     B2_TRY(upload_mask(idx, mask, st));
-    const void* q_dev = idx->q_in.p;
-    B2_TRY(adapt_queries(idx, q_dev, q_dtype, nq, st));
     B2_TRY(masked_search(idx, q_dev, q_dtype, nq, k, idx->mask_dev.as<uint32_t>(), 0, idx->out_sc.as<float>(),
                          idx->out_id.as<int64_t>(), st));
-    B2_CUDA(cudaMemcpyAsync(out_scores, idx->out_sc.p, (size_t)nq * k * sizeof(float), cudaMemcpyDeviceToHost, st));
-    B2_CUDA(cudaMemcpyAsync(out_idx, idx->out_id.p, (size_t)nq * k * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
-    cudaError_t e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) { set_error("masked search failed on the device: %s", cudaGetErrorString(e)); return B2_ECUDA; }
-    return B2_OK;
+    return download_topk(idx, nq, k, out_scores, out_idx, st);
 }
 
 int b2_index_range_search(b2_index* idx, const void* q, int64_t nq, int32_t q_dtype, float radius, const int64_t* ids, int64_t n_ids,
@@ -1218,30 +1126,12 @@ int b2_index_range_search(b2_index* idx, const void* q, int64_t nq, int32_t q_dt
     if (!idx->range) idx->range.reset(new RangeWork());
     RangeWork& W = *idx->range;
     idx->last_filter_ms = -1.f;
-    const size_t qbytes = (size_t)nq * idx->d * esize(q_dtype);
-    B2_TRY(idx->q_in.ensure(qbytes));
-    B2_CUDA(cudaMemcpyAsync(idx->q_in.p, q, qbytes, cudaMemcpyHostToDevice, st));
-    const void* q_dev = idx->q_in.p;
-    B2_TRY(adapt_queries(idx, q_dev, q_dtype, nq, st));
+    const void* q_dev = nullptr;
     const int64_t* ids_dev = nullptr;
-    if (ids) {
-        bool identity = n_ids == idx->n;
-        for (int64_t i = 0; identity && i < n_ids; ++i) identity = ids[i] == i;
-        if (!identity) {
-            B2_TRY(idx->ids_dev.ensure((size_t)std::max<int64_t>(n_ids, 1) * sizeof(int64_t)));
-            B2_CUDA(cudaMemcpyAsync(idx->ids_dev.p, ids, (size_t)n_ids * sizeof(int64_t), cudaMemcpyHostToDevice, st));
-            ids_dev = idx->ids_dev.as<int64_t>();
-        }
-    }
-    if (idx->host) {
-        B2_TRY(host_range(idx, W, q_dev, q_dtype, nq, radius, ids_dev ? ids : nullptr, ids_dev, n_ids, st));
-    } else if (ids_dev) {
-        MatView sub;
-        B2_TRY(build_subset(idx, ids_dev, n_ids, q_dtype, sub, st));
-        B2_TRY(range_device(idx, W, sub, q_dev, q_dtype, nq, radius, st));
-    } else {
-        B2_TRY(range_device(idx, W, idx->view, q_dev, q_dtype, nq, radius, st));
-    }
+    B2_TRY(stage_host_call(idx, q, nq, q_dtype, ids, n_ids, st, &q_dev, &ids_dev));
+    SearchRows R;
+    B2_TRY(select_rows(idx, ids, ids_dev, n_ids, q_dtype, st, &R));
+    B2_TRY(range_rows(idx, W, R, q_dev, q_dtype, nq, radius, st));
     B2_TRY(range_finish(W, ids_dev, 0, st));
     B2_CUDA(cudaMemcpyAsync(lims, W.lims.p, (size_t)(nq + 1) * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
     cudaError_t e = cudaStreamSynchronize(st);
@@ -1357,8 +1247,9 @@ int b2_index_search_stage2_packed_dev(b2_index* idx, const float* hint_dev, uint
     B2_TRY(idx->out_id.ensure((size_t)p.nq * p.k * sizeof(int64_t)));
     // uncertified queries: the exact local top-k (a superset of what the merge needs)
     int64_t n_sel = 0;
-    B2_TRY(certify(idx, p, p.chunks[0], idx->metric, nullptr, 0, idx->out_sc.as<float>(), idx->out_id.as<int64_t>(), hint_dev,
-                   /*fallback=*/true, &n_sel, st));
+    const FilterChunk& c = p.chunks[0];
+    B2_TRY(certify(idx, p, c, p.X, filter_lists(idx, p, c), idx->metric, nullptr, 0, idx->out_sc.as<float>(), idx->out_id.as<int64_t>(),
+                   hint_dev, /*fallback=*/true, &n_sel, st));
     B2_TRY(launch_pack_topk(idx->out_sc.as<float>(), idx->out_id.as<int64_t>(), p.nq * (int64_t)p.k, out_packed_dev, st));
     B2_CUDA(cudaStreamSynchronize(st));
     return B2_OK;
@@ -1477,78 +1368,47 @@ static int debug_filter_lists(b2_index* idx, const void* q, int64_t nq, int32_t 
         B2_TRY(upload_mask(idx, mask, st));
         mask_dev = idx->mask_dev.as<uint32_t>();
     }
-    if (idx->host) {
-        // a host-resident index: the folded lists after the last corpus chunk, the one list of `cap` entries finalize reads,
-        // reported as one split of two halves of cap / 2 (kp = cap) with its bound in both thr entries
-        if (top1) { set_error("the k-means assignment is not available on a host-resident index"); return B2_EINVAL; }
-        HostRows& H = idx->host->main;
-        const void* q_dev = nullptr;
-        if (lists) {
-            B2_TRY(idx->q_in.ensure((size_t)nq * idx->d * esize(q_dtype)));
-            B2_CUDA(cudaMemcpyAsync(idx->q_in.p, q, (size_t)nq * idx->d * esize(q_dtype), cudaMemcpyHostToDevice, st));
-            q_dev = idx->q_in.p;
-            B2_TRY(adapt_queries(idx, q_dev, q_dtype, nq, st));
-        }
-        FilterPlan p;
-        B2_TRY(host_plan(idx, H, q_dev, q_dtype, nq, k, level, p));
-        p.X.mask = mask_dev;
-        const int cap = p.use_filter ? finalize_capacity(p.kp, k) : 0;
-        const FilterChunk c = p.use_filter ? p.chunks[0] : FilterChunk();
-        plan[0] = cap ? 1 : 0;
-        plan[1] = cap;
-        plan[2] = 1;
-        plan[3] = 0;
-        plan[4] = c.cluster;
-        plan[5] = p.two_level ? 1 : 0;
-        plan[6] = p.X.filt_dtype;
-        plan[7] = (int32_t)p.chunks.size();
-        *rel_eps = p.rel_eps;
-        if (p.chunks.size() > 1) { set_error("%lld queries take %zu query chunks; one is supported", (long long)nq, p.chunks.size()); return B2_ERANGE; }
-        if (!lists || !cap) return B2_OK;
-        B2_TRY(stream_filter_fold(idx, H, p, c, idx->metric, cap, st));
-        HostStore& hs = *idx->host;
-        B2_CUDA(cudaMemcpyAsync(cand_score, hs.run_score.p, (size_t)nq * cap * sizeof(float), cudaMemcpyDeviceToHost, st));
-        B2_CUDA(cudaMemcpyAsync(cand_id, hs.run_id.p, (size_t)nq * cap * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-        B2_CUDA(cudaMemcpy2DAsync(cand_thr, 2 * sizeof(float), hs.run_thr.p, sizeof(float), sizeof(float), (size_t)nq, cudaMemcpyDeviceToHost, st));
-        B2_CUDA(cudaMemcpy2DAsync(cand_thr + 1, 2 * sizeof(float), hs.run_thr.p, sizeof(float), sizeof(float), (size_t)nq, cudaMemcpyDeviceToHost, st));
-        cudaError_t e = cudaStreamSynchronize(st);
-        if (e != cudaSuccess) { set_error("streamed filter failed on the device: %s", cudaGetErrorString(e)); return B2_ECUDA; }
-        return B2_OK;
-    }
-    MatView X = idx->view;
-    X.mask = mask_dev;
-    if (level == 1 || top1) X.filt16 = nullptr;  // the second level drops the bf16 copy; the k-means centroid view has none
-    const size_t qbytes = (size_t)nq * idx->d * esize(q_dtype);
+    if (idx->host && top1) { set_error("the k-means assignment is not available on a host-resident index"); return B2_EINVAL; }
     const void* q_dev = nullptr;
     if (lists) {
-        B2_TRY(idx->q_in.ensure(qbytes));
-        B2_CUDA(cudaMemcpyAsync(idx->q_in.p, q, qbytes, cudaMemcpyHostToDevice, st));
-        q_dev = idx->q_in.p;
-        B2_TRY(adapt_queries(idx, q_dev, q_dtype, nq, st));
-    } else if (q_dtype != B2_I8) {
+        const int64_t* no_ids = nullptr;
+        B2_TRY(stage_host_call(idx, q, nq, q_dtype, nullptr, 0, st, &q_dev, &no_ids));
+    } else if (q_dtype != B2_I8 && !idx->host) {
         B2_TRY(ensure_f16_copy(idx->view, idx->filt_f16, st));
     }
-    X.filt_f16 = idx->view.filt_f16;
-    X.filt_f16_pitch = idx->view.filt_f16_pitch;
+    SearchRows R;
+    B2_TRY(select_rows(idx, nullptr, nullptr, 0, q_dtype, st, &R));
+    R.X.mask = mask_dev;
+    if (level == 1 || top1) R.X.filt16 = nullptr;  // the second level drops the bf16 copy; the k-means centroid view has none
     FilterPlan p;
-    B2_TRY(plan_filter(X, q_dev, q_dtype, nq, k, top1 != 0, idx->device, p));
+    B2_TRY(plan_rows(idx, R, q_dev, q_dtype, nq, k, top1 != 0, level, p));
+    const int cap = R.H && p.use_filter ? finalize_capacity(p.kp, k) : 0;
     const FilterChunk c = p.use_filter ? p.chunks[0] : FilterChunk();
-    plan[0] = p.use_filter ? 1 : 0;
-    plan[1] = p.use_filter ? p.kp : 0;
-    plan[2] = c.n_splits;
-    plan[3] = c.units_whole;
+    // streamed rows: the folded lists after the last corpus chunk, the one list of `cap` entries finalize reads, reported as one
+    // split of two halves of cap / 2 (kp = cap) with its bound in both thr entries
+    const int kp = R.H ? cap : p.use_filter ? p.kp : 0;  // 0: no lists, the dense path answers
+    plan[0] = kp ? 1 : 0;
+    plan[1] = kp;
+    plan[2] = R.H ? 1 : c.n_splits;
+    plan[3] = R.H ? 0 : c.units_whole;
     plan[4] = c.cluster;
     plan[5] = p.two_level ? 1 : 0;
     plan[6] = p.X.filt_dtype;
     plan[7] = (int32_t)p.chunks.size();
     *rel_eps = p.rel_eps;
     if (p.chunks.size() > 1) { set_error("%lld queries take %zu query chunks; one is supported", (long long)nq, p.chunks.size()); return B2_ERANGE; }
-    if (!lists || !p.use_filter) return B2_OK;
-    B2_TRY(run_filter(idx, p, c, idx->metric, st));
-    const size_t entries = (size_t)nq * c.n_splits * p.kp;
-    B2_CUDA(cudaMemcpyAsync(cand_score, idx->cand_score.p, entries * sizeof(float), cudaMemcpyDeviceToHost, st));
-    B2_CUDA(cudaMemcpyAsync(cand_id, idx->cand_id.p, entries * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-    B2_CUDA(cudaMemcpyAsync(cand_thr, idx->cand_thr.p, (size_t)nq * c.n_splits * 2 * sizeof(float), cudaMemcpyDeviceToHost, st));
+    if (!lists || !kp) return B2_OK;
+    CandLists L;
+    B2_TRY(chunk_lists(idx, R, p, c, idx->metric, cap, &L, st));
+    const size_t entries = (size_t)nq * L.n_lists * L.list_len;
+    B2_CUDA(cudaMemcpyAsync(cand_score, L.score, entries * sizeof(float), cudaMemcpyDeviceToHost, st));
+    B2_CUDA(cudaMemcpyAsync(cand_id, L.id, entries * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    if (L.n_lists == 1) {
+        for (int h = 0; h < 2; ++h)
+            B2_CUDA(cudaMemcpy2DAsync(cand_thr + h, 2 * sizeof(float), L.thr, sizeof(float), sizeof(float), (size_t)nq, cudaMemcpyDeviceToHost, st));
+    } else {
+        B2_CUDA(cudaMemcpyAsync(cand_thr, L.thr, (size_t)nq * L.n_lists * sizeof(float), cudaMemcpyDeviceToHost, st));
+    }
     cudaError_t e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) { set_error("filter failed on the device: %s", cudaGetErrorString(e)); return B2_ECUDA; }
     return B2_OK;

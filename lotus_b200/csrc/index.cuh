@@ -120,7 +120,7 @@ struct PinnedBuf {
 };
 
 // Rows in pinned host memory plus what a streamed search needs of them on the device: norms, a bf16 copy for the first level of
-// an fp32 store, and the stream plan (host_resident.cu). Used for a host-resident index and for its large ids subsets.
+// an fp32 store, and the stream plan (api.cu). Used for a host-resident index and for its large ids subsets.
 struct HostRows {
     PinnedBuf rows;    // [n, d] in dtype, pitch d (what finalize, the dense path and gather read through UVA)
     PinnedBuf rows16;  // fp32 stores with n >= 4096: the bf16 rounding of the rows (first level), pitch d
@@ -243,7 +243,7 @@ struct b2_index {
     DevBuf mask_dev;  // masked search from host buffers: the row bitmap of the call
     b2_index* f16_twin = nullptr;  // int8 indexes: the fp16 copy k-means runs on (kmeans_view)
     // host-resident indexes (b2_index_create_host): the rows live in pinned, mapped host memory and searches stream them
-    // through a ring of device slots (host_resident.cu); `store` stays empty and `view.store` is the mapped pointer
+    // through a ring of device slots (api.cu); `store` stays empty and `view.store` is the mapped pointer
     std::unique_ptr<b2::HostStore> host;
     std::unique_ptr<b2::RangeWork> range;  // range search workspaces, made on the first range search
     ~b2_index();  // destroys the stream and events; the buffers free themselves
@@ -263,8 +263,17 @@ inline int refuse_host_resident(const b2_index* idx, const char* what) {
 // searchable view (filter operand, row norms, max norm) of a row-major device matrix
 int build_view(const void* store, int64_t n, int d, int dtype, DevBuf& filt_pad, DevBuf& norm2, DevBuf& scalar, MatView& v,
                cudaStream_t st, DevBuf* filt16 = nullptr);
-// the exact top-k pipeline on device buffers: wgmma filter -> finalize/certify -> dense fallback
-int search_core(b2_index* idx, const MatView& X, int metric, const void* q_dev, int q_dtype, int64_t nq, int k,
+// The rows a search reads: a device view (the whole index, a gathered ids subset, either with `mask` set), or rows in pinned
+// host memory that the search streams through the ring (H), X then being the view finalize and the dense path read through the
+// mapped pointer.
+struct SearchRows {
+    MatView X;
+    HostRows* H = nullptr;
+    SearchRows() = default;
+    SearchRows(const MatView& v) : X(v) {}  // a device view (k-means searches its centroid view)
+};
+// the exact top-k pipeline: wgmma filter -> finalize/certify -> dense fallback
+int search_core(b2_index* idx, const SearchRows& R, int metric, const void* q_dev, int q_dtype, int64_t nq, int k,
                 const int64_t* id_map, int64_t id_offset, float* out_sc, int64_t* out_id, cudaStream_t st, int level = 0);
 float filter_rel_eps(int store_dtype, int filt_dtype, int q_dtype, int d);
 // the index k-means runs on: idx itself, or for an int8 index its fp16 twin (exact), made on first use
