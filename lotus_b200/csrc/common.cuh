@@ -165,7 +165,8 @@ int launch_knn_filter(const MatView& X, const void* q_filt, int64_t q_pitch, int
                       int n_splits, int cluster, int workers, float* cand_score, int32_t* cand_id, float* cand_thr,
                       cudaStream_t stream, bool top1 = false, int units_whole = 0);
 int filter_cluster(int64_t nq, int64_t n, bool top1);  // CTAs per cluster of a filter launch: nq queries, n corpus rows
-int filter_workers(int device, int kp, int cl, int* workers);  // co-resident clusters of that launch on the current device
+int filter_workers(int device, int kp, int cl, int* workers);  // co-resident workers of that launch on the current device
+                                                               // (kp = 0: the range filter)
 int filter_choose_splits(int64_t nq, int64_t n, int workers, int cl, bool top1 = false, int min_splits = 1,
                          int* units_whole = nullptr);  // 0: impossible; *units_whole > 0: two-phase schedule (see the definition)
 int filter_min_splits_for_k(int k);
@@ -173,7 +174,6 @@ int sm_count(int device);  // multiprocessor count of a device, cached
 int launch_pair_filter(const MatView& X, float thr, int part, int nparts, int32_t* pair_i, int32_t* pair_j,
                        unsigned long long* pair_count, unsigned long long cap, int device, cudaStream_t stream);
 // range search: (query, row) candidates whose filter score beats thr[query] (NaN: none), see range.cu
-int range_filter_workers(int device, int cl, int* workers);
 int range_filter_splits(int64_t nq, int64_t n, int workers, int cl);
 int launch_range_filter(const MatView& X, const void* q_filt, int64_t q_pitch, int64_t nq, int metric, const float* thr, int cluster,
                         int workers, int2* cand, unsigned long long* count, unsigned long long cap, cudaStream_t stream);

@@ -322,7 +322,7 @@ struct FilterParams {
     int32_t num_kb;        // K-blocks per tile = ceil(d / elements per 64 B)
     int32_t n_mtiles;      // ceil(nq / 128)
     int32_t n_munits;      // schedulable query units: n_mtiles, or ceil(n_mtiles / 2) pairs of query tiles in cluster mode
-                           // (clusters of four: rounded so that the units cut into splits are even, see launch_knn_filter)
+                           // (clusters of four: rounded so that the units cut into splits are even, see filter_params)
     int32_t n_splits;
     int32_t top1;             // host-side switch only: the TOP1 kernel variant is launched (k-means assignment)
     int32_t tiles_per_split;  // corpus tiles (of 256 rows) per split
@@ -1178,90 +1178,41 @@ int make_tmap(CUtensorMap* map, const void* base, Op op, int64_t rows, int64_t c
     return B2_OK;
 }
 
-template <typename Kern, typename... Extra>
-int launch_cluster(Kern kern, int grid, int smem, int cl, const CUtensorMap& tq, const CUtensorMap& tx, const FilterParams& p,
-                   cudaStream_t stream, Extra... extra) {
-    // the attribute is per DEVICE (not per process): set it on every launch — a microsecond — so that a process driving
-    // several GPUs (B200VS(device=i) for several i) launches correctly on each of them
+// The launch config of `grid` CTAs in clusters of `cl` with `smem` bytes of dynamic shared memory each; *attr backs cfg->attrs.
+// Also raises kern's shared-memory limit to smem. The attribute is per DEVICE (not per process): it is set on every launch
+// — a microsecond — so that a process driving several GPUs (B200VS(device=i) for several i) launches correctly on each of them.
+template <typename Kern>
+int cluster_config(Kern kern, int grid, int cl, int smem, cudaStream_t stream, cudaLaunchConfig_t* cfg, cudaLaunchAttribute* attr) {
     B2_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)grid);
-    cfg.blockDim = dim3(NUM_THREADS);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = (unsigned)cl;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    B2_CUDA(cudaLaunchKernelEx(&cfg, kern, tq, tx, p, extra...));
-    B2_LAUNCH_CHECK();
-    g_stats[ST_FILTER_LAUNCHES]++;
+    *cfg = {};
+    cfg->gridDim = dim3((unsigned)grid);
+    cfg->blockDim = dim3(NUM_THREADS);
+    cfg->dynamicSmemBytes = smem;
+    cfg->stream = stream;
+    attr->id = cudaLaunchAttributeClusterDimension;
+    attr->val.clusterDim.x = (unsigned)cl;
+    attr->val.clusterDim.y = 1;
+    attr->val.clusterDim.z = 1;
+    cfg->attrs = attr;
+    cfg->numAttrs = 1;
     return B2_OK;
 }
 
-template <int KP, bool IS_L2, Op OP, int CL, bool TOP1 = false>
-int launch_variant(const CUtensorMap& tq, const CUtensorMap& tx, const FilterParams& p, int grid, cudaStream_t stream) {
-    return launch_cluster(knn_filter_kernel<KP, IS_L2, OP, CL, TOP1>, grid, smem_bytes(KP), CL, tq, tx, p, stream);
-}
-
-// the masked kernels (mask != nullptr): same grid, shared memory and schedule as the unmasked ones
-template <int KP, bool IS_L2, int CL>
-int launch_masked_op(Op op, const CUtensorMap& tq, const CUtensorMap& tx, const FilterParams& p, int grid, const uint32_t* mask,
-                     cudaStream_t stream) {
-    constexpr int SMEM = smem_bytes(KP);
-    switch (op) {
-        case Op::TF32: return launch_cluster(knn_masked_filter_kernel<KP, IS_L2, Op::TF32, CL>, grid, SMEM, CL, tq, tx, p, stream, mask);
-        case Op::BF16: return launch_cluster(knn_masked_filter_kernel<KP, IS_L2, Op::BF16, CL>, grid, SMEM, CL, tq, tx, p, stream, mask);
-        case Op::I8: return launch_cluster(knn_masked_i8_filter_kernel<KP, IS_L2, CL>, grid, SMEM, CL, tq, tx, p, stream, mask);
-        default: return launch_cluster(knn_masked_filter_kernel<KP, IS_L2, Op::F16, CL>, grid, SMEM, CL, tq, tx, p, stream, mask);  // Op::F16
-    }
-}
-
-template <int KP, bool IS_L2, int CL, bool TOP1 = false>
-int launch_op(Op op, const CUtensorMap& tq, const CUtensorMap& tx, const FilterParams& p, int grid, cudaStream_t stream) {
-    switch (op) {
-        case Op::TF32: return launch_variant<KP, IS_L2, Op::TF32, CL, TOP1>(tq, tx, p, grid, stream);
-        case Op::BF16: return launch_variant<KP, IS_L2, Op::BF16, CL, TOP1>(tq, tx, p, grid, stream);
-        case Op::I8:
-            if constexpr (TOP1) {
-                set_error("internal: no int8 top-1 filter (k-means does not take int8 points)");
-                return B2_EINVAL;
-            } else {
-                return launch_cluster(knn_i8_filter_kernel<KP, IS_L2, CL>, grid, smem_bytes(KP), CL, tq, tx, p, stream);
-            }
-        default: return launch_variant<KP, IS_L2, Op::F16, CL, TOP1>(tq, tx, p, grid, stream);  // Op::F16
-    }
-}
-
-template <int KP, int CL>
-int launch_kp(bool is_l2, Op op, const CUtensorMap& tq, const CUtensorMap& tx, const FilterParams& p, int grid,
-              const uint32_t* mask, cudaStream_t stream) {
-    if (mask)
-        return is_l2 ? launch_masked_op<KP, true, CL>(op, tq, tx, p, grid, mask, stream)
-                     : launch_masked_op<KP, false, CL>(op, tq, tx, p, grid, mask, stream);
-    return is_l2 ? launch_op<KP, true, CL>(op, tq, tx, p, grid, stream) : launch_op<KP, false, CL>(op, tq, tx, p, grid, stream);
-}
-
-// k == 1 (k-means assignment, KP = 16): register-resident top-2 epilogue
-template <int CL>
-int launch_top1(bool is_l2, Op op, const CUtensorMap& tq, const CUtensorMap& tx, const FilterParams& p, int grid,
-                cudaStream_t stream) {
-    return is_l2 ? launch_op<16, true, CL, true>(op, tq, tx, p, grid, stream)
-                 : launch_op<16, false, CL, true>(op, tq, tx, p, grid, stream);
-}
-
-template <int CL>
-int launch_cl(int kp, bool is_l2, Op op, const CUtensorMap& tq, const CUtensorMap& tx, const FilterParams& p, int grid,
-              const uint32_t* mask, cudaStream_t stream) {
-    switch (kp) {
-        case 16: return launch_kp<16, CL>(is_l2, op, tq, tx, p, grid, mask, stream);
-        case 32: return launch_kp<32, CL>(is_l2, op, tq, tx, p, grid, mask, stream);
-        case 64: return launch_kp<64, CL>(is_l2, op, tq, tx, p, grid, mask, stream);
-        case 72: return launch_kp<72, CL>(is_l2, op, tq, tx, p, grid, mask, stream);
-        default: set_error("internal: unsupported candidate capacity %d", kp); return B2_EINVAL;
+// Launches the filter entry `kern` (one of the *_entry selectors below) with the entry's arguments. A null entry is a
+// combination no kernel is instantiated for.
+template <typename Kern, typename... Args>
+int launch_cluster(Kern kern, int grid, int cl, int smem, cudaStream_t stream, const Args&... args) {
+    if constexpr (std::is_null_pointer_v<Kern>) {
+        set_error("internal: no filter kernel for this launch (top-1 takes no int8 points, no mask and at most CTA pairs)");
+        return B2_EINVAL;
+    } else {
+        cudaLaunchConfig_t cfg;
+        cudaLaunchAttribute attr;
+        B2_TRY(cluster_config(kern, grid, cl, smem, stream, &cfg, &attr));
+        B2_CUDA(cudaLaunchKernelEx(&cfg, kern, args...));
+        B2_LAUNCH_CHECK();
+        g_stats[ST_FILTER_LAUNCHES]++;
+        return B2_OK;
     }
 }
 
@@ -1270,18 +1221,9 @@ int launch_cl(int kp, bool is_l2, Op op, const CUtensorMap& tq, const CUtensorMa
 // trailing wave.
 template <typename Kern>
 int co_resident_clusters(Kern kern, int smem, int cl, int* n) {
-    B2_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)cl);
-    cfg.blockDim = dim3(NUM_THREADS);
-    cfg.dynamicSmemBytes = smem;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = (unsigned)cl;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
+    cudaLaunchConfig_t cfg;
+    cudaLaunchAttribute attr;
+    B2_TRY(cluster_config(kern, cl, cl, smem, nullptr, &cfg, &attr));
     *n = 0;
     B2_CUDA(cudaOccupancyMaxActiveClusters(n, kern, &cfg));
     if (*n <= 0) {
@@ -1291,14 +1233,136 @@ int co_resident_clusters(Kern kern, int smem, int cl, int* n) {
     return B2_OK;
 }
 
-// every instantiation of one KP has the same block, shared memory and register budget, so the IP / bf16 one stands for all
-template <int KP>
-int co_resident_filter_clusters(int cl, int* n) {
+// Runtime values to template arguments: each helper calls the generic lambda f once, with the value as a
+// std::integral_constant.
+template <typename F>
+int with_cluster(int cl, F&& f) {
     switch (cl) {
-        case 1: return co_resident_clusters(knn_filter_kernel<KP, false, Op::BF16, 1>, smem_bytes(KP), cl, n);
-        case 2: return co_resident_clusters(knn_filter_kernel<KP, false, Op::BF16, 2>, smem_bytes(KP), cl, n);
-        default: return co_resident_clusters(knn_filter_kernel<KP, false, Op::BF16, FILTER_CL>, smem_bytes(KP), cl, n);
+        case 1: return f(std::integral_constant<int, 1>{});
+        case 2: return f(std::integral_constant<int, 2>{});
+        case FILTER_CL: return f(std::integral_constant<int, FILTER_CL>{});
+        default: set_error("internal: unsupported cluster size %d", cl); return B2_EINVAL;
     }
+}
+
+template <typename F>
+int with_kp(int kp, F&& f) {
+    switch (kp) {
+        case 16: return f(std::integral_constant<int, 16>{});
+        case 32: return f(std::integral_constant<int, 32>{});
+        case 64: return f(std::integral_constant<int, 64>{});
+        case 72: return f(std::integral_constant<int, 72>{});
+        default: set_error("internal: unsupported candidate capacity %d", kp); return B2_EINVAL;
+    }
+}
+
+template <typename F>
+int with_op(Op op, F&& f) {
+    switch (op) {
+        case Op::TF32: return f(std::integral_constant<Op, Op::TF32>{});
+        case Op::BF16: return f(std::integral_constant<Op, Op::BF16>{});
+        case Op::I8: return f(std::integral_constant<Op, Op::I8>{});
+        default: return f(std::integral_constant<Op, Op::F16>{});  // Op::F16
+    }
+}
+
+template <typename F>
+int with_bool(bool b, F&& f) {
+    return b ? f(std::true_type{}) : f(std::false_type{});
+}
+
+// The __global__ of each filter family for one set of template arguments, nullptr where none is instantiated. These are
+// the only places that know that int8 has entries of its own (IGMMA, apart from the floating-point HGMMA kernels).
+// k == 1 (k-means assignment, KP = 16, CTA pairs at most): the register-resident top-2 epilogue; k-means takes no int8 points
+// and no mask.
+template <int KP, bool IS_L2, Op OP, int CL, bool TOP1>
+auto knn_entry() {
+    if constexpr (TOP1) {
+        if constexpr (KP == 16 && OP != Op::I8 && CL <= 2) return knn_filter_kernel<KP, IS_L2, OP, CL, true>;
+        else return nullptr;
+    } else if constexpr (OP == Op::I8) {
+        return knn_i8_filter_kernel<KP, IS_L2, CL>;
+    } else {
+        return knn_filter_kernel<KP, IS_L2, OP, CL>;
+    }
+}
+
+// the masked kernels (mask != nullptr): same grid, shared memory and schedule as the unmasked ones
+template <int KP, bool IS_L2, Op OP, int CL, bool TOP1>
+auto knn_masked_entry() {
+    if constexpr (TOP1) return nullptr;
+    else if constexpr (OP == Op::I8) return knn_masked_i8_filter_kernel<KP, IS_L2, CL>;
+    else return knn_masked_filter_kernel<KP, IS_L2, OP, CL>;
+}
+
+// the range filter keeps no list, so it has no KP
+template <Op OP, bool IS_L2, int CL>
+auto range_entry() {
+    if constexpr (OP == Op::I8) return range_i8_filter_kernel<IS_L2, CL>;
+    else return range_filter_kernel<OP, IS_L2, CL>;
+}
+
+// the all-pairs filter runs single CTAs or CTA pairs
+template <Op OP, int CL>
+auto pair_entry() {
+    if constexpr (CL > 2) return nullptr;
+    else if constexpr (OP == Op::I8) return pair_i8_filter_kernel<CL>;
+    else return pair_filter_kernel<OP, CL>;
+}
+
+// The checks every filter launch opens with: nq queries against the rows of X, no work (*empty) with fewer than min_rows.
+int filter_prologue(const MatView& X, int64_t nq, int64_t min_rows, bool is_l2, int cluster, int workers, bool* empty) {
+    *empty = nq <= 0 || X.n < min_rows;
+    if (*empty) return B2_OK;
+    if (X.n > 0x7fffff00LL || nq > 0x7fffff00LL) {
+        set_error("matrix too large for 32-bit row ids (n=%lld nq=%lld)", (long long)X.n, (long long)nq);
+        return B2_ERANGE;
+    }
+    if (is_l2 && (!X.norm2 || (filter_op(X.filt_dtype) == Op::I8 && !X.norm2_i8))) {
+        set_error("internal: L2 filter without row norms");
+        return B2_EINVAL;
+    }
+    // the two CTA pairs of a cluster of four sweep the same corpus tiles only with an even worker count
+    if ((cluster != 1 && cluster != 2 && cluster != FILTER_CL) || workers <= 0 || (cluster > 2 && workers % 2 != 0)) {
+        set_error("internal: bad filter launch (%d workers of %d CTAs)", workers, cluster);
+        return B2_EINVAL;
+    }
+    return B2_OK;
+}
+
+// The schedule geometry of a launch over nq queries and the rows of X in clusters of `cluster`: n_splits corpus splits, of
+// which the first units_whole query units (knn's two-phase schedule) take only the first. Every other field is zero.
+int filter_params(const MatView& X, Op op, int64_t nq, int cluster, int n_splits, int units_whole, FilterParams* out) {
+    FilterParams p{};
+    p.nq = (int32_t)nq;
+    p.n = (int32_t)X.n;
+    p.num_kb = (int32_t)ceil_div(X.d, KB_BYTES / op_bytes(op));
+    p.n_mtiles = (int32_t)ceil_div(nq, BLOCK_M);
+    p.n_munits = cluster > 1 ? (p.n_mtiles + 1) / 2 : p.n_mtiles;
+    p.n_ntiles = (int32_t)ceil_div(X.n, BLOCK_N);
+    p.tiles_per_split = (int32_t)ceil_div(p.n_ntiles, n_splits);
+    p.n_splits = n_splits;
+    p.units_whole = units_whole;
+    if ((int64_t)p.tiles_per_split * (n_splits - 1) >= p.n_ntiles) {
+        set_error("internal: empty corpus split (tiles %d, splits %d)", p.n_ntiles, n_splits);
+        return B2_EINVAL;
+    }
+    if (units_whole < 0 || units_whole > p.n_munits || (cluster > 2 && units_whole % 2 != 0)) {
+        set_error("internal: bad two-phase schedule (%d whole units of %d, clusters of %d)", units_whole, p.n_munits, cluster);
+        return B2_EINVAL;
+    }
+    // clusters of four: the two CTA pairs of a cluster sweep the same corpus tiles only with an even number of whole units and
+    // an even number of units cut into splits; a surplus unit past the last query tile loads zeros, writes nothing
+    if (cluster > 2) p.n_munits += (p.n_munits - units_whole) & 1;
+    *out = p;
+    return B2_OK;
+}
+
+// CTAs of a persistent launch: no more workers than work items (as the kernel's num_items counts them). Workers are CTA pairs
+// in cluster mode; in clusters of four both counts are even, so whole clusters are launched.
+int filter_grid(const FilterParams& p, int cluster, int workers) {
+    const int64_t items = p.pair_mode ? p.pair_items : (int64_t)p.units_whole + (int64_t)(p.n_munits - p.units_whole) * p.n_splits;
+    return (cluster > 1 ? 2 : 1) * (int)std::min<int64_t>(items, workers);
 }
 
 }  // namespace
@@ -1338,24 +1402,25 @@ int filter_cluster(int64_t nq, int64_t n, bool top1) {
     return mode == 1 && ceil_div(nq, BLOCK_M) >= cl ? cl : 1;
 }
 
-// Workers of one persistent filter launch with candidate capacity kp on the current device, which is `device`: as many as
-// are co-resident (CTA pairs in cluster mode, two per cluster of four; single CTAs otherwise), cached per device.
+// Workers of one persistent filter launch in clusters of `cl` on the current device, which is `device`: as many as are
+// co-resident (CTA pairs in cluster mode, two per cluster of four; single CTAs otherwise), cached per device. kp is the knn
+// filter's candidate capacity, 0 for the range filter. Every instantiation of one family and KP has the same block, shared
+// memory and register budget, so the IP / bf16 one stands for all.
 int filter_workers(int device, int kp, int cl, int* workers) {
-    static int cached[64][3][4] = {};
-    const int ki = kp == 16 ? 0 : kp == 32 ? 1 : kp == 64 ? 2 : 3;
+    static int cached[64][3][5] = {};
     const int ci = cl == 1 ? 0 : cl == 2 ? 1 : 2;
+    const int ki = kp == 0 ? 0 : kp == 16 ? 1 : kp == 32 ? 2 : kp == 64 ? 3 : 4;
     int* slot = (device >= 0 && device < 64) ? &cached[device][ci][ki] : nullptr;
     if (slot && *slot) {
         *workers = *slot;
         return B2_OK;
     }
-    switch (kp) {
-        case 16: B2_TRY(co_resident_filter_clusters<16>(cl, workers)); break;
-        case 32: B2_TRY(co_resident_filter_clusters<32>(cl, workers)); break;
-        case 64: B2_TRY(co_resident_filter_clusters<64>(cl, workers)); break;
-        case 72: B2_TRY(co_resident_filter_clusters<72>(cl, workers)); break;
-        default: set_error("internal: unsupported candidate capacity %d", kp); return B2_EINVAL;
-    }
+    B2_TRY(with_cluster(cl, [&](auto CL) {
+        if (kp == 0) return co_resident_clusters(range_filter_kernel<Op::BF16, false, CL.value>, RANGE_SMEM, CL, workers);
+        return with_kp(kp, [&](auto KP) {
+            return co_resident_clusters(knn_filter_kernel<KP.value, false, Op::BF16, CL.value>, smem_bytes(KP), CL, workers);
+        });
+    }));
     if (cl > 2) *workers *= cl / 2;
     if (slot) *slot = *workers;
     return B2_OK;
@@ -1421,87 +1486,45 @@ int filter_choose_splits(int64_t nq, int64_t n, int workers, int cl, bool top1, 
 int launch_knn_filter(const MatView& X, const void* q_filt, int64_t q_pitch, int64_t nq, int metric, int kp,
                       int n_splits, int cluster, int workers, float* cand_score, int32_t* cand_id, float* cand_thr,
                       cudaStream_t stream, bool top1, int units_whole) {
-    if (nq <= 0 || X.n <= 0) return B2_OK;
-    if (X.n > 0x7fffff00LL || nq > 0x7fffff00LL) {
-        set_error("matrix too large for 32-bit row ids (n=%lld nq=%lld)", (long long)X.n, (long long)nq);
-        return B2_ERANGE;
-    }
+    const bool is_l2 = metric == B2_METRIC_L2;
+    bool empty;
+    B2_TRY(filter_prologue(X, nq, 1, is_l2, cluster, workers, &empty));
+    if (empty) return B2_OK;
     const Op op = filter_op(X.filt_dtype);
-    const int kb_elems = KB_BYTES / op_bytes(op);
     CUtensorMap tq, tx;
-    const int64_t op_cols = X.d;
-    B2_TRY(make_tmap(&tq, q_filt, op, nq, op_cols, q_pitch, BLOCK_M));
+    B2_TRY(make_tmap(&tq, q_filt, op, nq, X.d, q_pitch, BLOCK_M));
     // each CTA of a cluster loads 1/cluster of the 256-row corpus tile (and multicasts it to all of them)
-    B2_TRY(make_tmap(&tx, X.filt, op, X.n, op_cols, X.filt_pitch, BLOCK_N / cluster));
+    B2_TRY(make_tmap(&tx, X.filt, op, X.n, X.d, X.filt_pitch, BLOCK_N / cluster));
     FilterParams p;
+    B2_TRY(filter_params(X, op, nq, cluster, n_splits, units_whole, &p));
     p.xnorm = X.norm2;
     p.xnorm_i = X.norm2_i8;
     p.cand_score = cand_score;
     p.cand_id = cand_id;
     p.cand_thr = cand_thr;
-    p.nq = (int32_t)nq;
-    p.n = (int32_t)X.n;
-    p.num_kb = (int32_t)ceil_div(X.d, kb_elems);
-    p.n_mtiles = (int32_t)ceil_div(nq, BLOCK_M);
-    p.n_munits = cluster > 1 ? (p.n_mtiles + 1) / 2 : p.n_mtiles;
-    p.n_ntiles = (int32_t)ceil_div(X.n, BLOCK_N);
-    p.tiles_per_split = (int32_t)ceil_div(p.n_ntiles, n_splits);
-    p.n_splits = n_splits;
-    p.units_whole = units_whole;
     p.top1 = (top1 && kp == 16) ? 1 : 0;  // register-resident top-2 epilogue: requested by the k-means assignment path only
-    p.pair_mode = 0;
-    p.part = 0;
     p.nparts = 1;
-    p.pair_thr = 0.f;
-    p.pair_i = p.pair_j = nullptr;
-    p.pair_count = nullptr;
-    p.pair_cap = 0;
-    if ((int64_t)p.tiles_per_split * (n_splits - 1) >= p.n_ntiles) {
-        set_error("internal: empty corpus split (tiles %d, splits %d)", p.n_ntiles, n_splits);
-        return B2_EINVAL;
-    }
-    if (units_whole < 0 || units_whole > p.n_munits) {
-        set_error("internal: bad two-phase schedule (%d whole units of %d)", units_whole, p.n_munits);
-        return B2_EINVAL;
-    }
-    if (cluster > 2) {
-        // the two CTA pairs of a cluster sweep the same corpus tiles only with an even worker count, an even number of whole
-        // units and an even number of units cut into splits: a surplus unit past the last query tile loads zeros, writes nothing
-        if (workers % 2 != 0 || units_whole % 2 != 0) {
-            set_error("internal: clusters of %d with %d workers and %d whole units", cluster, workers, units_whole);
-            return B2_EINVAL;
-        }
-        p.n_munits += (p.n_munits - units_whole) & 1;
-    }
-    const int64_t items = (int64_t)units_whole + (int64_t)(p.n_munits - units_whole) * n_splits;
     if (units_whole > 0 && n_splits > 1) {
         // whole units write split 0 only: the other lists of their queries must read as empty (id -1, bound -inf)
         B2_CUDA(cudaMemsetAsync(cand_id, 0xFF, (size_t)nq * n_splits * kp * sizeof(int32_t), stream));
         B2_TRY(launch_fill_f32(cand_thr, nq * (int64_t)n_splits * 2, -INFINITY, stream));
     }
-    const bool is_l2 = metric == B2_METRIC_L2;
-    if (is_l2 && (!X.norm2 || (op == Op::I8 && !X.norm2_i8))) {
-        set_error("internal: L2 filter without row norms");
-        return B2_EINVAL;
-    }
-    if ((cluster != 1 && cluster != 2 && (cluster != FILTER_CL || p.top1)) || workers <= 0) {
-        set_error("internal: bad filter launch (%d workers of %d CTAs)", workers, cluster);
-        return B2_EINVAL;
-    }
-    // workers are CTA pairs in cluster mode; in clusters of four both counts are even, so whole clusters are launched
-    const int grid = (cluster > 1 ? 2 : 1) * (int)std::min<int64_t>(items, workers);
-    if (p.top1) {
-        if (X.mask) {
-            set_error("internal: the k-means assignment takes no row mask");
-            return B2_EINVAL;
-        }
-        return cluster == 1 ? launch_top1<1>(is_l2, op, tq, tx, p, grid, stream) : launch_top1<2>(is_l2, op, tq, tx, p, grid, stream);
-    }
-    switch (cluster) {
-        case 1: return launch_cl<1>(kp, is_l2, op, tq, tx, p, grid, X.mask, stream);
-        case 2: return launch_cl<2>(kp, is_l2, op, tq, tx, p, grid, X.mask, stream);
-        default: return launch_cl<FILTER_CL>(kp, is_l2, op, tq, tx, p, grid, X.mask, stream);
-    }
+    const int grid = filter_grid(p, cluster, workers);
+    return with_cluster(cluster, [&](auto CL) {
+        return with_kp(kp, [&](auto KP) {
+            return with_bool(is_l2, [&](auto L2) {
+                return with_op(op, [&](auto OP) {
+                    return with_bool(p.top1, [&](auto TOP1) {
+                        if (X.mask)
+                            return launch_cluster(knn_masked_entry<KP.value, L2.value, OP.value, CL.value, TOP1.value>(), grid, CL,
+                                                  smem_bytes(KP), stream, tq, tx, p, X.mask);
+                        return launch_cluster(knn_entry<KP.value, L2.value, OP.value, CL.value, TOP1.value>(), grid, CL, smem_bytes(KP),
+                                              stream, tq, tx, p);
+                    });
+                });
+            });
+        });
+    });
 }
 
 // query tiles per dealing group of the all-pairs schedule: one per SM, so that one wave of CTAs is one group
@@ -1516,33 +1539,22 @@ static int pair_group_size(int device) {
 // capacity cap) in arbitrary order; *pair_count receives the total found.
 int launch_pair_filter(const MatView& X, float thr, int part, int nparts, int32_t* pair_i, int32_t* pair_j,
                        unsigned long long* pair_count, unsigned long long cap, int device, cudaStream_t stream) {
-    if (X.n <= 1) return B2_OK;
-    if (X.n > 0x7fffff00LL) {
-        set_error("matrix too large for 32-bit row ids (n=%lld)", (long long)X.n);
-        return B2_ERANGE;
-    }
+    static const bool two = [] { const char* e = getenv("B2_PAIR_2CTA"); return e ? atoi(e) != 0 : true; }();  // default: CTA pairs
+    const int cluster = two && ceil_div(X.n, BLOCK_M) >= 2 ? 2 : 1;
+    const int workers = sm_count(device) / cluster;
+    bool empty;
+    B2_TRY(filter_prologue(X, X.n, 2, false, cluster, workers, &empty));
+    if (empty) return B2_OK;
     const Op op = filter_op(X.filt_dtype);
-    const int kb_elems = KB_BYTES / op_bytes(op);
     CUtensorMap tq, tx;
     B2_TRY(make_tmap(&tq, X.filt, op, X.n, X.d, X.filt_pitch, BLOCK_M));
-    B2_TRY(make_tmap(&tx, X.filt, op, X.n, X.d, X.filt_pitch, BLOCK_N));
+    B2_TRY(make_tmap(&tx, X.filt, op, X.n, X.d, X.filt_pitch, BLOCK_N / cluster));  // each CTA of a pair stages half a corpus tile
     FilterParams p;
-    memset(&p, 0, sizeof(p));
-    p.nq = (int32_t)X.n;
-    p.n = (int32_t)X.n;
-    p.num_kb = (int32_t)ceil_div(X.d, kb_elems);
-    static const bool two = [] { const char* e = getenv("B2_PAIR_2CTA"); return e ? atoi(e) != 0 : true; }();  // default: CTA pairs
-    const bool two_cta = two && ceil_div(X.n, BLOCK_M) >= 2;
-    if (two_cta) B2_TRY(make_tmap(&tx, X.filt, op, X.n, X.d, X.filt_pitch, BLOCK_N / 2));  // each CTA stages half a corpus tile
-    p.n_mtiles = (int32_t)ceil_div(X.n, BLOCK_M);
-    p.n_munits = two_cta ? (p.n_mtiles + 1) / 2 : p.n_mtiles;
-    p.n_ntiles = (int32_t)ceil_div(X.n, BLOCK_N);
-    p.n_splits = 1;
-    p.tiles_per_split = p.n_ntiles;
+    B2_TRY(filter_params(X, op, X.n, cluster, 1, 0, &p));
     p.pair_mode = 1;
     p.part = part;
     p.nparts = nparts;
-    p.pair_group = two_cta ? std::max(1, pair_group_size(device) / 2) : pair_group_size(device);  // one unit per worker
+    p.pair_group = std::max(1, pair_group_size(device) / cluster);  // one unit per worker
     {
         const char* e = getenv("B2_PAIR_ALIGN");
         p.pair_align = e ? (atoi(e) != 0) : 1;
@@ -1559,84 +1571,10 @@ int launch_pair_filter(const MatView& X, float thr, int part, int nparts, int32_
     const int64_t items = my_full * p.pair_group + ((rem && full_groups % nparts == part) ? rem : 0);
     p.pair_items = (int32_t)items;
     if (items <= 0) return B2_OK;
-    const int grid = two_cta ? 2 * (int)std::min<int64_t>(items, sm_count(device) / 2) : (int)std::min<int64_t>(items, sm_count(device));
-    switch (op) {
-        case Op::TF32:
-            return two_cta ? launch_cluster(pair_filter_kernel<Op::TF32, 2>, grid, PAIR_SMEM, 2, tq, tx, p, stream)
-                           : launch_cluster(pair_filter_kernel<Op::TF32, 1>, grid, PAIR_SMEM, 1, tq, tx, p, stream);
-        case Op::BF16:
-            return two_cta ? launch_cluster(pair_filter_kernel<Op::BF16, 2>, grid, PAIR_SMEM, 2, tq, tx, p, stream)
-                           : launch_cluster(pair_filter_kernel<Op::BF16, 1>, grid, PAIR_SMEM, 1, tq, tx, p, stream);
-        case Op::I8:
-            return two_cta ? launch_cluster(pair_i8_filter_kernel<2>, grid, PAIR_SMEM, 2, tq, tx, p, stream)
-                           : launch_cluster(pair_i8_filter_kernel<1>, grid, PAIR_SMEM, 1, tq, tx, p, stream);
-        default:  // Op::F16
-            return two_cta ? launch_cluster(pair_filter_kernel<Op::F16, 2>, grid, PAIR_SMEM, 2, tq, tx, p, stream)
-                           : launch_cluster(pair_filter_kernel<Op::F16, 1>, grid, PAIR_SMEM, 1, tq, tx, p, stream);
-    }
-}
-
-namespace {
-
-template <typename Kern>
-int launch_range_cluster(Kern kern, int grid, int cl, const CUtensorMap& tq, const CUtensorMap& tx, const FilterParams& p,
-                         const RangeParams& rp, cudaStream_t stream) {
-    B2_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, RANGE_SMEM));
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)grid);
-    cfg.blockDim = dim3(NUM_THREADS);
-    cfg.dynamicSmemBytes = RANGE_SMEM;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = (unsigned)cl;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    B2_CUDA(cudaLaunchKernelEx(&cfg, kern, tq, tx, p, rp));
-    B2_LAUNCH_CHECK();
-    g_stats[ST_FILTER_LAUNCHES]++;
-    return B2_OK;
-}
-
-template <bool IS_L2, int CL>
-int launch_range_op(Op op, int grid, const CUtensorMap& tq, const CUtensorMap& tx, const FilterParams& p, const RangeParams& rp,
-                    cudaStream_t stream) {
-    switch (op) {
-        case Op::TF32: return launch_range_cluster(range_filter_kernel<Op::TF32, IS_L2, CL>, grid, CL, tq, tx, p, rp, stream);
-        case Op::BF16: return launch_range_cluster(range_filter_kernel<Op::BF16, IS_L2, CL>, grid, CL, tq, tx, p, rp, stream);
-        case Op::I8: return launch_range_cluster(range_i8_filter_kernel<IS_L2, CL>, grid, CL, tq, tx, p, rp, stream);
-        default: return launch_range_cluster(range_filter_kernel<Op::F16, IS_L2, CL>, grid, CL, tq, tx, p, rp, stream);  // Op::F16
-    }
-}
-
-template <int CL>
-int launch_range_cl(bool is_l2, Op op, int grid, const CUtensorMap& tq, const CUtensorMap& tx, const FilterParams& p,
-                    const RangeParams& rp, cudaStream_t stream) {
-    return is_l2 ? launch_range_op<true, CL>(op, grid, tq, tx, p, rp, stream) : launch_range_op<false, CL>(op, grid, tq, tx, p, rp, stream);
-}
-
-}  // namespace
-
-// Workers of one persistent range-filter launch in clusters of `cl` on the current device, which is `device` (CTA pairs in
-// cluster mode, two per cluster of four), cached per device.
-int range_filter_workers(int device, int cl, int* workers) {
-    static int cached[64][3] = {};
-    const int ci = cl == 1 ? 0 : cl == 2 ? 1 : 2;
-    int* slot = (device >= 0 && device < 64) ? &cached[device][ci] : nullptr;
-    if (slot && *slot) {
-        *workers = *slot;
-        return B2_OK;
-    }
-    switch (cl) {
-        case 1: B2_TRY(co_resident_clusters(range_filter_kernel<Op::BF16, false, 1>, RANGE_SMEM, 1, workers)); break;
-        case 2: B2_TRY(co_resident_clusters(range_filter_kernel<Op::BF16, false, 2>, RANGE_SMEM, 2, workers)); break;
-        default: B2_TRY(co_resident_clusters(range_filter_kernel<Op::BF16, false, FILTER_CL>, RANGE_SMEM, FILTER_CL, workers)); break;
-    }
-    if (cl > 2) *workers *= cl / 2;
-    if (slot) *slot = *workers;
-    return B2_OK;
+    const int grid = filter_grid(p, cluster, workers);
+    return with_cluster(cluster, [&](auto CL) {
+        return with_op(op, [&](auto OP) { return launch_cluster(pair_entry<OP.value, CL.value>(), grid, CL, PAIR_SMEM, stream, tq, tx, p); });
+    });
 }
 
 // Corpus splits of a range filter: items carry no list, so a split costs no warm-up; the corpus is cut only as far as it
@@ -1653,54 +1591,34 @@ int range_filter_splits(int64_t nq, int64_t n, int workers, int cl) {
 
 // Candidates (query, row) of a range search: rows of X whose filter score beats thr[query] (filter-score space, see
 // RangeParams). cand (device, capacity cap) receives them in arbitrary order and *count (device, zeroed by the caller) the
-// total found, which may exceed cap. cluster / workers as filter_cluster / range_filter_workers chose them.
+// total found, which may exceed cap. cluster / workers as filter_cluster / filter_workers chose them.
 int launch_range_filter(const MatView& X, const void* q_filt, int64_t q_pitch, int64_t nq, int metric, const float* thr, int cluster,
                         int workers, int2* cand, unsigned long long* count, unsigned long long cap, cudaStream_t stream) {
-    if (nq <= 0 || X.n <= 0) return B2_OK;
-    if (X.n > 0x7fffff00LL || nq > 0x7fffff00LL) {
-        set_error("matrix too large for 32-bit row ids (n=%lld nq=%lld)", (long long)X.n, (long long)nq);
-        return B2_ERANGE;
-    }
-    const Op op = filter_op(X.filt_dtype);
-    const int kb_elems = KB_BYTES / op_bytes(op);
     const bool is_l2 = metric == B2_METRIC_L2;
-    if (is_l2 && (!X.norm2 || (op == Op::I8 && !X.norm2_i8))) {
-        set_error("internal: L2 range filter without row norms");
-        return B2_EINVAL;
-    }
-    if ((cluster != 1 && cluster != 2 && cluster != FILTER_CL) || workers <= 0 || (cluster > 2 && workers % 2 != 0)) {
-        set_error("internal: bad range filter launch (%d workers of %d CTAs)", workers, cluster);
-        return B2_EINVAL;
-    }
+    bool empty;
+    B2_TRY(filter_prologue(X, nq, 1, is_l2, cluster, workers, &empty));
+    if (empty) return B2_OK;
+    const Op op = filter_op(X.filt_dtype);
     CUtensorMap tq, tx;
     B2_TRY(make_tmap(&tq, q_filt, op, nq, X.d, q_pitch, BLOCK_M));
     B2_TRY(make_tmap(&tx, X.filt, op, X.n, X.d, X.filt_pitch, BLOCK_N / cluster));
     FilterParams p;
-    memset(&p, 0, sizeof(p));
+    B2_TRY(filter_params(X, op, nq, cluster, range_filter_splits(nq, X.n, workers, cluster), 0, &p));
     p.xnorm = X.norm2;
     p.xnorm_i = X.norm2_i8;
-    p.nq = (int32_t)nq;
-    p.n = (int32_t)X.n;
-    p.num_kb = (int32_t)ceil_div(X.d, kb_elems);
-    p.n_mtiles = (int32_t)ceil_div(nq, BLOCK_M);
-    p.n_munits = cluster > 1 ? (p.n_mtiles + 1) / 2 : p.n_mtiles;
-    p.n_munits += cluster > 2 ? (p.n_munits & 1) : 0;  // clusters of four: an even number of units (a surplus one writes nothing)
-    p.n_ntiles = (int32_t)ceil_div(X.n, BLOCK_N);
-    p.n_splits = range_filter_splits(nq, X.n, workers, cluster);
-    p.tiles_per_split = (int32_t)ceil_div(p.n_ntiles, p.n_splits);
-    p.units_whole = 0;
     RangeParams rp;
     rp.thr = thr;
     rp.cand = cand;
     rp.count = count;
     rp.cap = cap;
-    const int64_t items = (int64_t)p.n_munits * p.n_splits;
-    const int grid = (cluster > 1 ? 2 : 1) * (int)std::min<int64_t>(items, workers);
-    switch (cluster) {
-        case 1: return launch_range_cl<1>(is_l2, op, grid, tq, tx, p, rp, stream);
-        case 2: return launch_range_cl<2>(is_l2, op, grid, tq, tx, p, rp, stream);
-        default: return launch_range_cl<FILTER_CL>(is_l2, op, grid, tq, tx, p, rp, stream);
-    }
+    const int grid = filter_grid(p, cluster, workers);
+    return with_cluster(cluster, [&](auto CL) {
+        return with_bool(is_l2, [&](auto L2) {
+            return with_op(op, [&](auto OP) {
+                return launch_cluster(range_entry<OP.value, L2.value, CL.value>(), grid, CL, RANGE_SMEM, stream, tq, tx, p, rp);
+            });
+        });
+    });
 }
 
 }  // namespace b2

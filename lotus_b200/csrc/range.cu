@@ -261,7 +261,7 @@ int range_begin(b2_index* idx, RangeWork& W, const MatView& X, int metric, const
         B2_TRY(launch_prep_queries(q_dev, q_dtype, nq, X.d, idx->q_filt.p, W.filt_dtype, W.q_pitch, st));
         W.q_filt = idx->q_filt.p;
         W.cluster = filter_cluster(nq, X.n, false);
-        B2_TRY(range_filter_workers(idx->device, W.cluster, &W.workers));
+        B2_TRY(filter_workers(idx->device, 0, W.cluster, &W.workers));
     }
     return B2_OK;
 }
