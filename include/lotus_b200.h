@@ -187,6 +187,15 @@ B2_API int b2_index_search_stage2_packed_dev(b2_index* idx, const float* hint_de
  * because cap < *n_results; the caller then retries with cap = *n_results. Every index residency and dtype. */
 B2_API int b2_index_range_search(b2_index* idx, const void* q, int64_t nq, int32_t q_dtype, float radius, const int64_t* ids,
                                  int64_t n_ids, int64_t* lims, float* out_d, int64_t* out_i, int64_t cap, int64_t* n_results);
+/* Masked range search: b2_index_range_search over the rows a bitmap selects, searched in place. mask is laid out as for
+ * b2_index_search_masked (ceil(n / 32) little-endian words, bits at or past n ignored). The result equals b2_index_range_search
+ * with ids = the ascending list of the set rows, bit for bit (lims, ids and score bits; an all-zero mask gives lims of zeros),
+ * and the argument checks, the NaN radius and B2_ERANGE behave as there. No copy of the subset is made: the range filter
+ * sweeps all n rows and only selected rows become candidates, so the candidate buffer scales with the hits among them.
+ * Every dtype, both metrics, both residencies. HOST buffers. */
+B2_API int b2_index_range_search_masked(b2_index* idx, const void* q, int64_t nq, int32_t q_dtype, float radius,
+                                        const uint32_t* mask, int64_t* lims, float* out_d, int64_t* out_i, int64_t cap,
+                                        int64_t* n_results);
 
 /* ---- row gather (faiss_vs.py:38-41) ------------------------------------------------------------------ */
 /* out[m,d] in the index's dtype = x[ids]; HOST out unless out_on_device != 0 (then ids is a device pointer too) */
@@ -280,8 +289,9 @@ B2_API int b2_debug_stream_times(const b2_index* idx, float* out4);
  * B2_BF16 / B2_F16 = 2-byte wgmma) with queries of `q_dtype`, dimension d. abs_eps is non-zero only where an operand is
  * rounded to fp16 (its subnormal spacing). For testing; the search paths use the same function. */
 B2_API int b2_debug_filter_eps(int32_t store_dtype, int32_t filt_dtype, int32_t q_dtype, int32_t d, float* rel_eps, float* abs_eps);
-/* The last b2_index_range_search of this handle: out4[0] the most candidates one range-filter launch produced (the peak size
- * of the candidate buffer), [1] the hits, [2] the queries the exact dense path answered, [3] 1 if the filter ran. */
+/* The last b2_index_range_search or b2_index_range_search_masked of this handle: out4[0] the most candidates one range-filter
+ * launch produced (the peak size of the candidate buffer), [1] the hits, [2] the queries the exact dense path answered, [3] 1
+ * if the filter ran. */
 B2_API int b2_debug_range_stats(const b2_index* idx, int64_t* out4);
 
 /* ---- instrumentation ---------------------------------------------------------------------------------- */

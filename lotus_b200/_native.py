@@ -25,7 +25,7 @@ SYMBOLS = [
     "b2_connected_components", "b2_kmeans", "b2_kmeans_assign", "b2_kmeans_accumulate", "b2_kmeans_assign_dev", "b2_kmeans_accumulate_dev", "b2_stats", "b2_stats_reset", "b2_last_filter_ms", "b2_host_f32_to_bf16", "b2_host_bf16_to_f32", "b2_debug_filter_plan",
     "b2_debug_filter_lists", "b2_debug_filter_eps", "b2_index_create_host", "b2_index_resident", "b2_debug_stream_plan",
     "b2_debug_stream_times", "b2_index_range_search", "b2_debug_range_stats",
-    "b2_index_search_masked", "b2_index_search_masked_dev", "b2_debug_filter_lists_masked",
+    "b2_index_search_masked", "b2_index_search_masked_dev", "b2_debug_filter_lists_masked", "b2_index_range_search_masked",
 ]
 
 
@@ -93,6 +93,8 @@ def lib() -> ctypes.CDLL:
     L.b2_index_search_stage2_packed_dev.argtypes = [vp, vp, vp, vp]
     L.b2_index_range_search.restype = c.c_int
     L.b2_index_range_search.argtypes = [vp, vp, i64, i32, f32, vp, i64, vp, vp, vp, i64, c.POINTER(i64)]
+    L.b2_index_range_search_masked.restype = c.c_int
+    L.b2_index_range_search_masked.argtypes = [vp, vp, i64, i32, f32, vp, vp, vp, vp, i64, c.POINTER(i64)]
     L.b2_debug_range_stats.restype = c.c_int
     L.b2_debug_range_stats.argtypes = [vp, c.POINTER(i64)]
     L.b2_index_gather.restype = c.c_int
@@ -397,15 +399,34 @@ class Index:
         if nq and q.shape[1] != self.d:
             raise ValueError(f"query dimension {q.shape[1]} != index dimension {self.d}")
         ids_a = None if ids is None else np.ascontiguousarray(ids, dtype=np.int64)
+        return self._range_call(nq, cap, lambda lims, D, I, cap, total: lib().b2_index_range_search(
+            self._h, _ptr(q) if nq else None, nq, q_dtype, float(radius), _ptr(ids_a), 0 if ids_a is None else len(ids_a),
+            _ptr(lims), _ptr(D), _ptr(I), cap, total))
+
+    def range_search_masked(self, q: np.ndarray, radius: float, q_dtype: int, mask, cap: Optional[int] = None):
+        """range_search(q, radius, q_dtype, ids=np.flatnonzero(mask)), bit for bit, without a gathered copy of the subset: the
+        range filter sweeps the whole index and only the selected rows become candidates. mask: bool[n], or packed uint32
+        words (pack_mask). Hits are reported by row id."""
+        q = np.ascontiguousarray(q)
+        nq = q.shape[0]
+        if nq and q.shape[1] != self.d:
+            raise ValueError(f"query dimension {q.shape[1]} != index dimension {self.d}")
+        words = pack_mask(mask, self.n)
+        return self._range_call(nq, cap, lambda lims, D, I, cap, total: lib().b2_index_range_search_masked(
+            self._h, _ptr(q) if nq else None, nq, q_dtype, float(radius), _ptr(words) if self.n else None,
+            _ptr(lims), _ptr(D), _ptr(I), cap, total))
+
+    @staticmethod
+    def _range_call(nq: int, cap: Optional[int], call):
+        """Runs call(lims, D, I, cap, byref(total)) of a range search entry point into host buffers, once more with the exact
+        size when the result outgrows `cap`, and returns (lims, D, I)."""
         lims = np.zeros(nq + 1, dtype=np.int64)
         cap = int(cap) if cap is not None else max(1 << 16, 64 * nq)
         for attempt in range(2):
             D = np.empty(cap, dtype=np.float32)
             I = np.empty(cap, dtype=np.int64)
             total = ctypes.c_int64(0)
-            rc = lib().b2_index_range_search(self._h, _ptr(q) if nq else None, nq, q_dtype, float(radius), _ptr(ids_a),
-                                             0 if ids_a is None else len(ids_a), _ptr(lims), _ptr(D), _ptr(I), cap,
-                                             ctypes.byref(total))
+            rc = call(lims, D, I, cap, ctypes.byref(total))
             if rc == ERANGE and attempt == 0 and total.value > cap:
                 cap = int(total.value)
                 continue
@@ -415,7 +436,7 @@ class Index:
         return lims, D[:m].copy(), I[:m].copy()
 
     def range_stats(self) -> dict:
-        """Counts of the last range_search (b2_debug_range_stats)."""
+        """Counts of the last range_search or range_search_masked (b2_debug_range_stats)."""
         out = (ctypes.c_int64 * 4)()
         check(lib().b2_debug_range_stats(self._h, out))
         return {"candidates_peak": out[0], "hits": out[1], "dense_queries": out[2], "filtered": bool(out[3])}

@@ -1107,8 +1107,11 @@ int b2_index_search_masked(b2_index* idx, const void* q, int64_t nq, int32_t q_d
     return download_topk(idx, nq, k, out_scores, out_idx, st);
 }
 
-int b2_index_range_search(b2_index* idx, const void* q, int64_t nq, int32_t q_dtype, float radius, const int64_t* ids, int64_t n_ids,
-                          int64_t* lims, float* out_d, int64_t* out_i, int64_t cap, int64_t* n_results) {
+// The range search of the ids subset (ids, n_ids), or of the rows a bitmap selects (mask: ceil(n / 32) host words), or of the
+// whole index. A masked search reads the rows in place; its candidates and dense rows are selected rows only, reported by
+// their positions in the index.
+static int range_search(b2_index* idx, const void* q, int64_t nq, int32_t q_dtype, float radius, const int64_t* ids, int64_t n_ids,
+                        const uint32_t* mask, int64_t* lims, float* out_d, int64_t* out_i, int64_t cap, int64_t* n_results) {
     if (!idx) { set_error("Index not loaded"); return B2_EINVAL; }
     if (nq < 0 || (nq > 0 && !q)) { set_error("bad query batch"); return B2_EINVAL; }
     if (!dtype_valid(q_dtype)) { set_error("q_dtype must be B2_F32, B2_BF16, B2_F16 or B2_I8"); return B2_EINVAL; }
@@ -1131,6 +1134,10 @@ int b2_index_range_search(b2_index* idx, const void* q, int64_t nq, int32_t q_dt
     B2_TRY(stage_host_call(idx, q, nq, q_dtype, ids, n_ids, st, &q_dev, &ids_dev));
     SearchRows R;
     B2_TRY(select_rows(idx, ids, ids_dev, n_ids, q_dtype, st, &R));
+    if (mask) {
+        B2_TRY(upload_mask(idx, mask, st));
+        R.X.mask = idx->mask_dev.as<uint32_t>();
+    }
     B2_TRY(range_rows(idx, W, R, q_dev, q_dtype, nq, radius, st));
     B2_TRY(range_finish(W, ids_dev, 0, st));
     B2_CUDA(cudaMemcpyAsync(lims, W.lims.p, (size_t)(nq + 1) * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
@@ -1150,6 +1157,18 @@ int b2_index_range_search(b2_index* idx, const void* q, int64_t nq, int32_t q_dt
         if (e != cudaSuccess) { set_error("range search failed on the device: %s", cudaGetErrorString(e)); return B2_ECUDA; }
     }
     return B2_OK;
+}
+
+int b2_index_range_search(b2_index* idx, const void* q, int64_t nq, int32_t q_dtype, float radius, const int64_t* ids, int64_t n_ids,
+                          int64_t* lims, float* out_d, int64_t* out_i, int64_t cap, int64_t* n_results) {
+    return range_search(idx, q, nq, q_dtype, radius, ids, n_ids, nullptr, lims, out_d, out_i, cap, n_results);
+}
+
+int b2_index_range_search_masked(b2_index* idx, const void* q, int64_t nq, int32_t q_dtype, float radius, const uint32_t* mask,
+                                 int64_t* lims, float* out_d, int64_t* out_i, int64_t cap, int64_t* n_results) {
+    if (!idx && b2_device_count() == 0) { set_error("no CUDA device: libb2lotus has no CPU fallback"); return B2_ENODEV; }
+    if (idx && !mask && idx->n > 0) { set_error("mask is NULL"); return B2_EINVAL; }
+    return range_search(idx, q, nq, q_dtype, radius, nullptr, 0, mask, lims, out_d, out_i, cap, n_results);
 }
 
 int b2_debug_range_stats(const b2_index* idx, int64_t* out4) {

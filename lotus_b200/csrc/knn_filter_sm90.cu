@@ -1018,9 +1018,14 @@ struct RangeParams {
 constexpr int RANGE_STAGES = MAX_STAGES;
 constexpr int RANGE_SMEM = RANGE_STAGES * STAGE_BYTES + BAR_BYTES + SMEM_ALIGN_SLACK;
 
-template <Op OP, bool IS_L2, int CL>
+// MASKED (masked range search): only the rows whose bit is set in `row_mask` (ceil(p.n / 32) words, laid out as for
+// knn_filter_body) can become candidates, so the candidates scale with the hits among the selected rows. A tile whose 256
+// bits are clear skips its epilogue (its stages are consumed all the same), a chunk whose 16 bits are clear is skipped, and
+// each column's bit is ANDed with the column-range test, so bits at or past p.n (the next chunk's, on a streamed chunk)
+// select nothing.
+template <Op OP, bool IS_L2, int CL, bool MASKED = false>
 __device__ __forceinline__ void range_filter_body(const CUtensorMap& tmap_q, const CUtensorMap& tmap_x, const FilterParams& p,
-                                                  const RangeParams& rp) {
+                                                  const RangeParams& rp, const uint32_t* row_mask = nullptr) {
     using AccT = std::conditional_t<OP == Op::I8, int32_t, float>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = align_smem(smem_raw);
@@ -1052,16 +1057,32 @@ __device__ __forceinline__ void range_filter_body(const CUtensorMap& tmap_q, con
                 else thr[h] = tq;
             }
             for (int t = t0; t < t1; ++t) {
+                if constexpr (MASKED) {  // the tile's 32 bytes of mask, on their way while the wgmmas run
+                    if (lane == 0) asm volatile("prefetch.global.L1 [%0];" ::"l"(row_mask + t * (BLOCK_N / 32)));
+                }
                 mma_tile<OP, RANGE_STAGES, CL, 0>(acc, no_afrag, false, ring, p.num_kb, g, sc.cta, stage, phase);
                 const int col0 = t * BLOCK_N + 2 * (lane & 3);
+                uint32_t mword = 0;  // MASKED: word (lane & 7) of the tile's mask, zero past the last word of the corpus
+                if constexpr (MASKED) {
+                    const int w = t * (BLOCK_N / 32) + (lane & 7);
+                    if (w < (p.n + 31) >> 5) mword = __ldg(row_mask + w);
+                    if (!__any_sync(0xffffffffu, mword != 0)) continue;  // no selected row in this tile
+                }
 #pragma unroll
                 for (int c = 0; c < BLOCK_N / 16; ++c) {  // 16-column chunks: acc[8c .. 8c + 7]
+                    // MASKED: bit i set = column 16 c + i of the tile is a selected row (the same for every lane)
+                    uint32_t live = 0xffffu;
+                    if constexpr (MASKED) {
+                        live = (__shfl_sync(0xffffffffu, mword, c >> 1) >> (16 * (c & 1))) & 0xffffu;
+                        if (live == 0) continue;  // warp-uniform: nothing selected in this chunk
+                    }
                     uint32_t mask = 0;
 #pragma unroll
                     for (int h = 0; h < 8; ++h) {
                         const int i = 8 * c + h;
                         const int gj = col0 + 8 * (i >> 2) + (i & 1);
-                        const bool valid = gj < p.n;
+                        bool valid = gj < p.n;
+                        if constexpr (MASKED) valid = valid && ((live >> (8 * (h >> 2) + (h & 1) + 2 * (lane & 3))) & 1u) != 0;
                         bool pass;
                         if constexpr (OP == Op::I8) {
                             pass = valid && i8_score<IS_L2>(acc[i], p, gj, valid) > thr[(i >> 1) & 1];
@@ -1115,6 +1136,22 @@ __global__ void __launch_bounds__(NUM_THREADS, 1)
 range_i8_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_x, const FilterParams p,
                        const RangeParams rp) {
     range_filter_body<Op::I8, IS_L2, CL>(tmap_q, tmap_x, p, rp);
+}
+
+// the masked range filter (masked range search): entries of their own, so that the kernels of an unmasked range search are
+// untouched. mask: ceil(p.n / 32) words, see range_filter_body
+template <Op OP, bool IS_L2, int CL>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+range_masked_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_x,
+                           const FilterParams p, const RangeParams rp, const uint32_t* __restrict__ mask) {
+    range_filter_body<OP, IS_L2, CL, true>(tmap_q, tmap_x, p, rp, mask);
+}
+
+template <bool IS_L2, int CL>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+range_masked_i8_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_x,
+                              const FilterParams p, const RangeParams rp, const uint32_t* __restrict__ mask) {
+    range_filter_body<Op::I8, IS_L2, CL, true>(tmap_q, tmap_x, p, rp, mask);
 }
 
 // ---- host side ---------------------------------------------------------------------------------------------
@@ -1300,6 +1337,12 @@ template <Op OP, bool IS_L2, int CL>
 auto range_entry() {
     if constexpr (OP == Op::I8) return range_i8_filter_kernel<IS_L2, CL>;
     else return range_filter_kernel<OP, IS_L2, CL>;
+}
+
+template <Op OP, bool IS_L2, int CL>
+auto range_masked_entry() {
+    if constexpr (OP == Op::I8) return range_masked_i8_filter_kernel<IS_L2, CL>;
+    else return range_masked_filter_kernel<OP, IS_L2, CL>;
 }
 
 // the all-pairs filter runs single CTAs or CTA pairs
@@ -1591,7 +1634,8 @@ int range_filter_splits(int64_t nq, int64_t n, int workers, int cl) {
 
 // Candidates (query, row) of a range search: rows of X whose filter score beats thr[query] (filter-score space, see
 // RangeParams). cand (device, capacity cap) receives them in arbitrary order and *count (device, zeroed by the caller) the
-// total found, which may exceed cap. cluster / workers as filter_cluster / filter_workers chose them.
+// total found, which may exceed cap. cluster / workers as filter_cluster / filter_workers chose them. With X.mask set (a masked
+// range search) only the selected rows become candidates.
 int launch_range_filter(const MatView& X, const void* q_filt, int64_t q_pitch, int64_t nq, int metric, const float* thr, int cluster,
                         int workers, int2* cand, unsigned long long* count, unsigned long long cap, cudaStream_t stream) {
     const bool is_l2 = metric == B2_METRIC_L2;
@@ -1615,6 +1659,9 @@ int launch_range_filter(const MatView& X, const void* q_filt, int64_t q_pitch, i
     return with_cluster(cluster, [&](auto CL) {
         return with_bool(is_l2, [&](auto L2) {
             return with_op(op, [&](auto OP) {
+                if (X.mask)
+                    return launch_cluster(range_masked_entry<OP.value, L2.value, CL.value>(), grid, CL, RANGE_SMEM, stream, tq, tx, p, rp,
+                                          X.mask);
                 return launch_cluster(range_entry<OP.value, L2.value, CL.value>(), grid, CL, RANGE_SMEM, stream, tq, tx, p, rp);
             });
         });

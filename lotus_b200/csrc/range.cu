@@ -5,9 +5,11 @@
 //                         filter's error margin, so that no row whose canonical result passes can score at or below it. A
 //                         query whose margin is not finite gets NaN (no filter candidates) and is listed for the dense path.
 //   range filter        : knn_filter_sm90.cu (range_filter_kernel): (query, row) pairs whose filter score beats the threshold.
+//                         A masked range search (b2_index_range_search_masked) runs range_masked_filter_kernel, which emits
+//                         selected rows only.
 //   range_verify_kernel : one warp per (query, row) pair: the canonical score (canonical.cuh, the arithmetic finalize uses)
 //                         and the strict comparison; a passing pair becomes a hit (query, position, score). The dense path is
-//                         the same kernel over every row of a query.
+//                         the same kernel over every row of a query (every selected row, in a masked search).
 //   assembly            : one radix sort of the hits by (query << 32 | position), lims by binary search, unpack to D / I.
 #include <cub/cub.cuh>
 
@@ -71,6 +73,7 @@ struct VerifyParams {
     const int32_t* dense_sel;  // dense mode (cand == nullptr): every row of [own_lo, n) for each of the n_dense queries
     int64_t n_dense;
     int64_t own_lo;  // rows below own_lo belong to an earlier pass (the re-streamed tail of a host-resident chunk)
+    const uint32_t* mask;  // masked range search: bit j is row j of this pass; the dense mode skips the cleared rows (null: none)
     int64_t base;    // position reported for row 0
     int32_t* hit_q;
     int32_t* hit_pos;
@@ -105,6 +108,7 @@ __global__ void range_verify_kernel(const VerifyParams p) {
         } else {
             qi = p.dense_sel[t / rows];
             j = p.own_lo + t % rows;
+            if (p.mask && !((p.mask[j >> 5] >> (j & 31)) & 1u)) continue;  // (warp-uniform)
         }
         if (j < p.own_lo) continue;  // (warp-uniform)
         if (qi != cur) {
@@ -280,6 +284,7 @@ int range_pass(b2_index* idx, RangeWork& W, const MatView& X, int64_t pitch, int
     vp.radius = W.radius;
     vp.own_lo = own_lo;
     vp.base = base;
+    vp.mask = X.mask;  // the filter of a masked search reads it too, so its candidates are selected rows only
     if (W.use_filter && W.n_dense < W.nq) {
         unsigned long long* count = W.counts.as<unsigned long long>();
         if (W.cand.cap < sizeof(int2)) B2_TRY(W.cand.ensure((size_t)std::max<int64_t>(1 << 20, 64 * W.nq) * sizeof(int2)));

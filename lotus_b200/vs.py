@@ -246,6 +246,20 @@ class MultiDeviceIndex:
         parts = list(self.pool.map(one, range(len(self.shards))))
         return combine_range_hits(nq, [p[0] for p in parts], [p[1] for p in parts], [p[2] for p in parts], ids_a)
 
+    def range_search_masked(self, q: np.ndarray, radius: float, q_dtype: int, mask):
+        """As `_native.Index.range_search_masked`: every shard searches its rows under its slice of the bitmap (built on the
+        host: shard bounds need not fall on word boundaries); the hits are then ordered per query by row id."""
+        words = nv.pack_mask(mask, self.n)
+        nq = len(q)
+
+        def one(g):
+            lo, hi = self.bounds[g]
+            lims, D, I = self.shards[g].range_search_masked(q, radius, q_dtype, nv.slice_mask(words, self.n, lo, hi))
+            return np.repeat(np.arange(nq, dtype=np.int64), np.diff(lims)), D, I + lo
+
+        parts = list(self.pool.map(one, range(len(self.shards))))
+        return combine_range_hits(nq, [p[0] for p in parts], [p[1] for p in parts], [p[2] for p in parts])
+
     def gather(self, ids) -> np.ndarray:
         ids = np.asarray(ids, dtype=np.int64)
         if len(ids) and (ids.min() < 0 or ids.max() >= self.n):
@@ -361,17 +375,19 @@ class B200VS(VS):
     memory, same results bit for bit; threshold_pairs / kmeans, hence sem_dedup / sem_cluster_by, raise ValueError) or
     "auto" (device when the store's device footprint plus a 1 GiB margin fits in free device memory, host otherwise;
     `resident(index_dir)` reports the choice). CUDA tensors given to a host-resident store are copied to the host.
-    subset: how `__call__(..., ids=...)` searches a subset of the rows. "gather" (default): a temporary index over a gathered
-    copy of vecs[ids], as the reference does. "mask": when ids is strictly ascending (what a pandas filter leaves) the whole
-    index is swept under a row bitmap instead, with the same result bit for bit, no copy of the subset in device memory and,
-    on a host-resident index, no gather on the host; any other ids (permuted or repeating: different tie order) take the
-    gathered path. "auto": the bitmap, for a strictly ascending ids, where the gathered copy is what hurts: on a
-    host-resident index when the subset does not fit its ring (it would be gathered on the host), on a device-resident one
-    when the copy's footprint plus a 1 GiB margin does not fit in free device memory (the gathered search would fail with
-    an allocation error). Everywhere else the gathered search was the faster one in bench_masked.py (H100 80GB HBM3 at a
+    subset: how `__call__(..., ids=...)` and `range_search(..., ids=...)` search a subset of the rows. "gather" (default): a
+    temporary index over a gathered copy of vecs[ids], as the reference does. "mask": when ids is strictly ascending (what a
+    pandas filter leaves) the whole index is swept under a row bitmap instead, with the same result bit for bit, no copy of
+    the subset in device memory and, on a host-resident index, no gather on the host; any other ids (permuted or repeating:
+    different tie order) take the gathered path. "auto": the bitmap, for a strictly ascending ids, where the gathered copy is
+    what hurts: on a host-resident index when the subset does not fit its ring (it would be gathered on the host), on a
+    device-resident one when the copy's footprint plus a 1 GiB margin does not fit in free device memory (the gathered
+    search would fail with an allocation error). Everywhere else the gathered search was the faster one in bench_masked.py (H100 80GB HBM3 at a
     700 W power limit, 1M x 768, subsets of 90 % down to 1 % of the rows: a masked search sweeps every row whatever the
     subset's size), so "auto" keeps it there; on the host-resident index the bitmap won for the subsets of 90 % and 50 %,
-    the ones larger than its 384 MB ring.
+    the ones larger than its 384 MB ring. Range search follows the same rule: bench_range_masked.py on the same card and
+    shapes found the same split (the bitmap slower at every share on the device-resident index, faster for the 90 % and
+    50 % subsets on the host-resident one).
     """
 
     accepts_id_arrays = True  # `ids=` may be a numpy int64 array (the operators then skip building a Python list)
@@ -612,17 +628,30 @@ class B200VS(VS):
         """faiss IndexFlat.range_search(x, radius) over the loaded index: (lims[Q+1] int64, D float32, I int64), query i's
         hits at [lims[i], lims[i+1]) in ascending id. IP keeps rows whose score is strictly greater than `radius`; L2 those
         whose squared distance is strictly less. D holds the values __call__ reports. ids: only those rows, as a temporary
-        index over vecs[ids] (faiss_vs.py:57-72): hits follow the order of `ids`, a repeated id once per occurrence. Queries
-        as __call__ accepts them."""
+        index over vecs[ids] (faiss_vs.py:57-72): hits follow the order of `ids`, a repeated id once per occurrence; `subset`
+        decides, as for __call__, whether a strictly ascending ids is searched under a row bitmap instead (same result).
+        Queries as __call__ accepts them."""
+        ids_a = None if ids is None else np.asarray(list(ids) if not isinstance(ids, np.ndarray) else ids, dtype=np.int64)
+        return self._range(query_vectors, radius, ids=ids_a)
+
+    def range_search_masked(self, query_vectors: Any, radius: float, mask: Any):
+        """range_search(query_vectors, radius, ids=np.flatnonzero(mask)) for callers that hold a boolean column rather than
+        ids: the rows whose entry of `mask` (bool, one per row of the index) is set, always searched under the bitmap."""
+        return self._range(query_vectors, radius, mask=np.asarray(mask, dtype=np.bool_))
+
+    def _range(self, query_vectors: Any, radius: float, ids: "np.ndarray | None" = None, mask: Any = None):
         if self.b2_index is None or self.index_dir is None:
             raise ValueError("Index not loaded")
-        ids_a = None if ids is None else np.asarray(list(ids) if not isinstance(ids, np.ndarray) else ids, dtype=np.int64)
         q, code, _ = _to_host_matrix(query_vectors, False, exact_bf16_ok=self.b2_index.dtype == nv.BF16, scratch=self._scratch,
                                      pass_f16=True, pass_i8=True)
         if q.shape[1] != self.b2_index.d:
             raise ValueError(f"query dimension {q.shape[1]} does not match the index dimension {self.b2_index.d}")
         try:
-            return self.b2_index.range_search(q, float(radius), code, ids=ids_a)
+            if ids is not None and self._subset_by_mask(ids):
+                mask = nv.ids_to_mask(ids, self.b2_index.n)
+            if mask is None:
+                return self.b2_index.range_search(q, float(radius), code, ids=ids)
+            return self.b2_index.range_search_masked(q, float(radius), code, mask)
         except nv.NativeError as e:
             if e.code in (nv.EINVAL, nv.ERANGE):
                 raise ValueError(e.msg) from e
